@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the Cold-Diffusion hot path on B200 (contract: see the task brief).
+"""bench.py -- headline benchmark of the Cold-Diffusion hot path on H100.
 
     python bench.py --gpus 1 --steps 5 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -17,12 +17,15 @@ inside a timed region.
 
 Both arms print the SAME `metric` string, unit and workload so that the driver can divide them.  The reference arm
 (`--impl reference`) times the reference algorithm (oracle/: the eager-PyTorch restatement of the reference's p_losses, 200-step
-Python q_sample loop included; the reference itself is Python under /root/reference and does not exist on the GPU box) on the host
+Python q_sample loop included) on the host
 cores at a bounded batch per step.  The same restatement on cuda:0 at the full micro-batch of 32 -- how the reference is deployed,
-cuDNN / cuBLAS eager -- is measured once per single-GPU run and reported as `reference_eager_b200` (the comparator SURVEY 8d
-calls the real bar).  The sampling half of the metric is one complete `GaussianDiffusion.sample(batch_size=32, img=...)` call of
+cuDNN / cuBLAS eager -- is measured once per single-GPU run and reported as `reference_eager`.  The sampling half of the metric is one complete `GaussianDiffusion.sample(batch_size=32, img=...)` call of
 200 reverse steps through the public API (`sample`).  `op_profile` is the in-situ time per C-ABI entry point of one step.
 All kernels run in their default configuration (no start-up tuning).
+
+--dump-outputs DIR writes what the last timed step computed: its loss (loss.npy, float64) and a fixed, seeded sample of 2^20 of
+the updated model parameters (params_sample.npy, float32, in named_parameters() order), so that two builds can be compared
+output for output.  Inputs and weights are seeded: the same arguments give the same inputs on every run.
 """
 import argparse
 import json
@@ -46,7 +49,7 @@ def read_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, 'measured'
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0), 'fallback'
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0), 'H100 SXM data sheet (dense, 700 W)'
 
 
 class ClockSampler(threading.Thread):
@@ -78,8 +81,7 @@ class ClockSampler(threading.Thread):
 
 
 # ------------------------------------------------------------------------------------------------------
-# reference arm / cpu baseline: the reference algorithm (oracle port; the reference itself is pure Python
-# under /root/reference, absent on the GPU box) on the host cores
+# reference arm / cpu baseline: the reference algorithm (oracle port) on the host cores
 # ------------------------------------------------------------------------------------------------------
 def cpu_train_sample(batch=2, steps=1, warmup=0, threads=None, device='cpu'):
     """times p_losses forward + backward + Adam of config 3 with the eager-PyTorch restatement of the reference (oracle/) at a
@@ -107,8 +109,8 @@ def cpu_train_sample(batch=2, steps=1, warmup=0, threads=None, device='cpu'):
     times = []
     tried = ''
     if calibrate:
-        # eager PyTorch on "all cores" of a many-core host can be far slower than on a few (round 1 measured 0.059 images/s with 128
-        # threads on the GPU box against ~0.9 with 8 threads elsewhere): one untimed step per candidate thread count, keep the fastest
+        # eager PyTorch on "all cores" of a many-core host can be far slower than on a few: one untimed step per candidate
+        # thread count, keep the fastest
         best = None
         for n in sorted({c for c in (8, 16, 32, 64, avail) if c <= avail} or {avail}):
             torch.set_num_threads(n)
@@ -182,6 +184,20 @@ def _timed_loop(fn, n, sync):
     return e0.elapsed_time(e1)
 
 
+def dump_outputs(out_dir, loss, model, n_sample=1 << 20):
+    """loss.npy (float64) and params_sample.npy: n_sample entries, at indices drawn with a fixed seed, of the concatenation of
+    the model's parameters in named_parameters() order (float32)"""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, 'loss.npy'), np.asarray(loss.detach().double().cpu().numpy(), dtype=np.float64))
+    flat = torch.cat([p.detach().reshape(-1).float() for _, p in model.named_parameters()])
+    n = flat.numel()
+    idx = np.sort(np.random.default_rng(0).choice(n, size=min(n, n_sample), replace=False))
+    sample = flat[torch.from_numpy(idx).to(flat.device)].cpu().numpy().astype(np.float32)
+    np.save(os.path.join(out_dir, 'params_sample.npy'), sample)
+
+
 # ------------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -193,6 +209,8 @@ def main():
     ap.add_argument('--no-sample', action='store_true', help='skip the 200-step sample() measurement (quick runs)')
     ap.add_argument('--no-others', action='store_true', help='skip the other BASELINE configs and the eager comparator (quick runs)')
     ap.add_argument('--no-autotune', action='store_true', help='accepted for compatibility; there is no start-up tuning any more')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the loss and a seeded sample of the updated parameters of the last timed step as DIR/<name>.npy')
     ap.add_argument('--reference-device', default='cpu', choices=['cpu', 'cuda'],
                     help="--impl reference only: 'cpu' (the contract) or 'cuda' = the same eager-PyTorch restatement on the GPU (informational)")
     args = ap.parse_args()
@@ -229,7 +247,7 @@ def main():
     B, A = C3['batch'], C3['accum']
     img_per_step = B * A
 
-    # distinct batches so consecutive steps never re-read the same inputs; activations (>3 GB/step) exceed the 126 MB L2
+    # distinct batches so consecutive steps never re-read the same inputs; activations (>3 GB/step) exceed the 50 MB L2
     g = torch.Generator().manual_seed(1234 + rank)
     nb = 4
     host = [torch.rand(B, 3, 128, 128, generator=g).mul_(2).sub_(1).pin_memory() for _ in range(nb * A)]
@@ -249,9 +267,12 @@ def main():
             ms = tt.item()
         return ms
 
+    last_loss = []
+
     def step_resident(s):
-        trainer.train_step(batches=[resident[(s * A + i) % (nb * A)] for i in range(A)])
+        loss = trainer.train_step(batches=[resident[(s * A + i) % (nb * A)] for i in range(A)])
         trainer.step += 1
+        last_loss[:] = [loss]
 
     losses = []
     loss_host = [torch.zeros((), dtype=torch.float32).pin_memory() for _ in range(2)]
@@ -280,6 +301,8 @@ def main():
     _lib.reset_launch_count()
     ms = timed(step_resident, K)
     launches = _lib.launch_count()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_loss[0], unet)
     for s in range(2):                      # untimed: first use of the pinned batches / loss buffers / events of the end-to-end path
         wl = trainer.train_step(batches=[host[(s * A + i) % (nb * A)] for i in range(A)])
         trainer.step += 1
@@ -322,7 +345,7 @@ def main():
             eager = {"error": repr(e)[:200]}
         torch.cuda.empty_cache()
 
-    # ---- roofline of the dominant kernel (tcgen05 tap-list convolution), CUDA events around every launch --------
+    # ---- roofline of the dominant kernel (wgmma tap-list convolution), CUDA events around every launch --------
     peaks, peak_kind = read_peaks()
     roof = None
     eng = unet.engine
@@ -335,19 +358,10 @@ def main():
         tot_fl = sum(f for (a, b, f) in eng.profile_convs)
         n_launch = len(eng.profile_convs)
         eng.profile_convs = None
-        tf32_peak = peaks['bf16_tflops_sustained'] / 2.0     # kind::tf32 runs at half the bf16 rate
+        tf32_peak = peaks['bf16_tflops_sustained'] / 2.0     # TF32 runs at half the bf16 rate
         ach = tot_fl / (tot_ms / 1e3) / 1e12
-        traffic, traffic_src = None, None
-        for name in ('conv_tc_traffic_r02.json', 'conv_tc_traffic_r01.json'):
-            try:
-                with open(os.path.join(ROOT, 'profiles', name)) as f:
-                    traffic, traffic_src = json.load(f)['dram_bytes_per_launch'], name
-                break
-            except Exception:
-                pass
-        roof = {"bound": "tensor", "kernel": "conv_tc_kernel / conv_tc2_kernel / conv_tc4_kernel (tcgen05 kind::tf32 implicit GEMM; fwd + dgrad launches)",
-                "achieved": ach, "peak": tf32_peak, "unit": "TFLOP/s", "frac": ach / tf32_peak, "traffic": traffic,
-                "traffic_unit": "DRAM bytes per launch (ncu capture of one step, profiles/%s)" % traffic_src,
+        roof = {"bound": "tensor", "kernel": "conv_tc_kernel (wgmma tf32 implicit GEMM; fwd + dgrad launches)",
+                "achieved": ach, "peak": tf32_peak, "unit": "TFLOP/s", "frac": ach / tf32_peak,
                 "peak_source": "%s bf16_tflops_sustained / 2 (TF32 rate)" % peak_kind, "launches_timed": n_launch,
                 "share_of_step_ms": tot_ms / (ms / K)}
 
@@ -387,7 +401,7 @@ def main():
                        "net": "Unet(dim=64, dim_mults=(1,2,4,8), channels=3)", "T": 200, "blur": "Exponential_reflect k=15 std=0.01",
                        "global_batch": img_per_step * world, "parallelism": "dp%d" % world,
                        "micro_batches": "%d x %d, gradients accumulated" % (A, B),
-                       "l2": "inputs rotate over 4 distinct batch sets; per-step activations (>3 GB) exceed the 126 MB L2"},
+                       "l2": "inputs rotate over 4 distinct batch sets; per-step activations (>3 GB) exceed the 50 MB L2"},
             "e2e": {"value": e2e, "unit": "images/s", "h2d_bytes_per_step": img_per_step * 3 * 128 * 128 * 4,
                     "d2h_bytes_per_step": 4, "ms_per_step": ms_e2e / K, "last_loss": losses[-1] if losses else None,
                     "losses_read": len(losses),
@@ -396,7 +410,7 @@ def main():
             "gpu_launches": launches,
             "roofline": roof,
             "cpu_baseline": cpu,
-            "reference_eager_b200": eager,
+            "reference_eager": eager,
             "clocks": sampler.summary() if sampler else None,
             "train_tflops": value * TRAIN_GFLOP_PER_IMG / 1e3,
             "other_configs": others,

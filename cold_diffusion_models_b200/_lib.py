@@ -52,12 +52,12 @@ class RepackJob(C.Structure):          # CdRepackJob (include/colddiff.h): one r
 
 
 lib.cd_version.restype = C.c_int
-if os.environ.get('COLDDIFF_2CTA') in ('0', '1', '2'):   # SM-pair (cta_group::2) convolution kernel, csrc/conv_tc2.cu; library default 1
+if os.environ.get('COLDDIFF_2CTA') in ('0', '1', '2'):   # SM-pair (two-CTA cluster) convolution kernel; library default 0
     lib.cd_conv_tc_set_2cta(int(os.environ['COLDDIFF_2CTA']))
 lib.cd_last_error.argtypes = [C.c_char_p, C.c_size_t]
 if os.environ.get('COLDDIFF_CONV_TWO_CTAS') in ('0', '64', '128', '192'):   # two CTAs per SM for the N <= 128 convolution tiles (bit mask)
     lib.cd_conv_tc_set_two_ctas(int(os.environ['COLDDIFF_CONV_TWO_CTAS']))
-if os.environ.get('COLDDIFF_CONV_HALO') in ('0', '1', '2', '3', '6'):   # halo-tile kernels for the 3x3 convolutions (1: csrc/conv_tc3.cu, 2: conv_tc4.cu)
+if os.environ.get('COLDDIFF_CONV_HALO') in ('0', '1', '2', '3', '6'):   # halo-tile kernel for the 3x3 convolutions (1: 16 x 8 tiles, 2: 16 x 16)
     lib.cd_conv_tc_set_halo(int(os.environ['COLDDIFF_CONV_HALO']))
 if os.environ.get('COLDDIFF_2CTA_BN') in ('0', '64', '128', '192'):   # N tiles below 256 on the SM-pair kernel (bit mask 128 | 64)
     lib.cd_conv_tc_set_2cta_bn(int(os.environ['COLDDIFF_2CTA_BN']))

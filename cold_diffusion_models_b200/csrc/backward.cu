@@ -211,8 +211,7 @@ __global__ void colsum_batched_kernel(const float* __restrict__ x, int ld, long 
 
 // float4 variant (opt-in, the image-edge switch cd_conv_simt_set_preload; C % 4 == 0, 16-byte aligned rows): a warp covers 32/G rows x
 // G channel quads (G = min(32, C/4) rounded up to a power of two), four independent 16-byte loads per thread in flight, partial
-// sums meet in shared memory, one atomicAdd per channel and block.  (The scalar kernel above reads the 1.3 GB of one step at
-// 1.5 TB/s.)  Different summation order than the scalar kernel: results agree to fp32 rounding.
+// sums meet in shared memory, one atomicAdd per channel and block.  Different summation order than the scalar kernel: results agree to fp32 rounding.
 __global__ void __launch_bounds__(256)
 colsum_batched_vec_kernel(const float* __restrict__ x, int ld, long long rows, int C, float* __restrict__ out, int out_ld,
                           long long rows_per_block, int G) {
@@ -313,8 +312,7 @@ attn_bwd_small_kernel(const float* __restrict__ dweff, const float* __restrict__
 //                 dv[n][he] = sum_d P[n][h,d] dctxn[h,d][e]
 // Two 32x32 GEMMs per head and pixel.  Block = kKvTiles tiles of 32 pixels of one image; dctxn is staged once per block in
 // both orientations, P and v of a tile transposed ([channel][pixel]) so that a thread owning 4 pixels x 4 channels feeds
-// 32 FMAs from 4 LDS.128 per step (the first version issued 2 scalar LDS per FMA and was shared-memory-issue bound:
-// 924 us at 128x128 against ~230 us of HBM traffic).
+// 32 FMAs from 4 LDS.128 per step (2 scalar LDS per FMA would make the kernel shared-memory-issue bound).
 constexpr int kKvPix = 32;
 constexpr int kKvTiles = 8;
 constexpr int kKvStride = 36;         // floats per channel row of the transposed tiles (16-byte aligned, 4-way store conflicts)
@@ -581,7 +579,7 @@ extern "C" int cd_layernorm_bwd(const float* dy, int dy_ld, const float* h, int 
   const int nq = C / 4;
   CD_REQUIRE((nq & (nq - 1)) == 0 || nq >= 32, "cd_layernorm_bwd: C/4 must be a power of two below 128 channels (C=%d)", C);
   // pixels per block: at most 512, but never fewer than ~4 blocks per SM (8192 pixels of the 16x16 level gave 16 blocks)
-  int ppb = static_cast<int>(npix / (148 * 4));
+  int ppb = static_cast<int>(npix / (cd_num_sms() * 4));
   if (ppb > 512) ppb = 512;
   if (ppb < 32) ppb = 32;
   const int blocks = cd_cdiv(npix, ppb);
@@ -626,7 +624,7 @@ extern "C" int cd_colsum_batched(const float* x, int ld, int B, int64_t rows, in
     const int nq = C / 4;
     int G = 1; while (G < nq && G < 32) G <<= 1;
     const int xb = cd_cdiv(nq, G);
-    long long rpbv = rows * xb * B / (148 * 4);          // >= 4 blocks per SM over the whole batch
+    long long rpbv = rows * xb * B / (cd_num_sms() * 4);          // >= 4 blocks per SM over the whole batch
     if (rpbv > 1024) rpbv = 1024;
     if (rpbv < 64) rpbv = 64;
     dim3 gv(xb, cd_cdiv(rows, rpbv), B);
@@ -665,7 +663,7 @@ extern "C" int cd_linattn_bwd_kv(const float* qkv, int ld, int B, int n, const f
     attr = true;
   }
   // tiles per block: up to kKvTiles (amortises the 32 KB dctxn staging), fewer when that would leave SMs idle
-  int tiles = static_cast<int>(static_cast<long long>(cd_cdiv(n, kKvPix)) * B / (148 * 2));
+  int tiles = static_cast<int>(static_cast<long long>(cd_cdiv(n, kKvPix)) * B / (cd_num_sms() * 2));
   if (tiles > kKvTiles) tiles = kKvTiles;
   if (tiles < 1) tiles = 1;
   dim3 grid(cd_cdiv(n, kKvPix * tiles), B);
@@ -707,10 +705,10 @@ extern "C" int cd_conv1x1_to_nchw_bwd(const float* dout_nchw, const float* x, in
 extern "C" int cd_small_gemm(const float* A, int lda, int transA, const float* Bm, int ldb, int transB,
                              float* Cm, int ldc, int M, int N, int K, int accumulate, void* stream) {
   const long long total = static_cast<long long>(M) * N;
-  if (K >= 512 && total <= 148 * 128) {
+  if (K >= 512 && total <= cd_num_sms() * 128) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (!accumulate) CD_CUDA(cudaMemset2DAsync(Cm, sizeof(float) * ldc, 0, sizeof(float) * N, M, st));
-    const int ks = cd_cdiv(148 * 4, cd_cdiv(total, 128));
+    const int ks = cd_cdiv(cd_num_sms() * 4, cd_cdiv(total, 128));
     const int kslice = cd_cdiv(K, ks);
     dim3 grid(cd_cdiv(total, 128), cd_cdiv(K, kslice));
     small_gemm_splitk_kernel<<<grid, 128, 0, st>>>(A, lda, transA, Bm, ldb, transB, Cm, ldc, M, N, K, kslice);

@@ -1,4 +1,4 @@
-// Internal helpers shared by the libcolddiff translation units (sm_100a only).
+// Internal helpers shared by the libcolddiff translation units (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda.h>
@@ -8,9 +8,9 @@
 #include "../../include/colddiff.h"
 
 #ifndef CD_HOST_ONLY
-#if !defined(__CUDA_ARCH__) || (__CUDA_ARCH__ >= 1000)
+#if !defined(__CUDA_ARCH__) || (__CUDA_ARCH__ >= 900)
 #else
-#error "libcolddiff is written for sm_100a only"
+#error "libcolddiff is written for sm_90a only"
 #endif
 #endif
 
@@ -23,6 +23,18 @@ void cd_set_error(const char* fmt, ...);
 #define CD_LAUNCH_CHECK() CD_CUDA(cudaGetLastError())
 
 static inline int cd_cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// SM count of the current device for the grid-size heuristics of the CUDA-core kernels (queried once; 132 = H100 SXM if the
+// query fails, which only changes how work is split)
+static inline int cd_num_sms() {
+  static int n = 0;
+  if (n <= 0) {
+    int dev = 0, v = 0;
+    n = (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0)
+            ? v : 132;
+  }
+  return n;
+}
 
 // conv_simt.cu / final_proj.cu: opt-in variants of the image-edge kernels (cd_conv_simt_set_preload)
 int cd_conv_simt_preload_enabled();

@@ -1,19 +1,18 @@
 // Line-coalesced epilogue of the tensor-core convolutions (opt-in, cd_conv_tc_set_staged_epilogue).
 //
-// After tcgen05.ld a lane holds 32 consecutive output channels of ITS OWN pixel, so the default epilogue writes "rows":
-// every store instruction of a warp touches 32 different 128-byte lines with one 32-byte sector each.  The short-K
-// convolutions (1x1 projections, K = 64..512) are bound by exactly that: the 128x128-pixel qkv projection writes 805 MB
-// in 508 us = 1.6 TB/s, 83 tiles per SM at ~11.7 k clocks per 64 KB tile against 512 clocks of MMAs
-// (profiles/conv_shapes_2cta_r01b.txt); going from 128-bit to 256-bit row stores already bought 10 % of the whole
-// convolution time, i.e. the cost follows the number of memory requests, not the bytes.
+// The default epilogue of conv_tc_kernel stores straight from the wgmma accumulator fragment: a lane holds pairs of adjacent
+// channels of two pixels, so every store instruction of a warp touches 8 different pixel rows with 32 bytes each.  The short-K
+// convolutions (1x1 projections, K = 64..512) do little MMA work per output byte, and there the number of memory requests,
+// not the bytes, can bound the launch.
 //
-// Here the 32 x 32 block of a warp goes through a per-warp shared-memory tile (row stride 36 floats: the float4 row
+// With this epilogue the accumulator chunk of a warpgroup is first staged so that a lane holds 32 consecutive output channels
+// of ITS OWN pixel (conv_tc.cu), and then the 32 x 32 block of a warp goes through a per-warp shared-memory tile (row stride 36 floats: the float4 row
 // writes and the float4 transposed reads are both conflict-free per quarter-warp) and leaves as 8 store instructions that
 // each cover 4 pixels x 128 contiguous bytes (4 full lines instead of 32 sectors in 32 lines); the residual / GELU'
 // operand reads are coalesced the same way.  The arithmetic per element and its order are those of the row epilogue
 // (acc + bias + resid -> out2 -> activation -> TF32 rounding -> out): results are bit-identical.
 //
-// No tcgen05 / TMA in this header: tests/simt_cpu executes it from source on the CPU (tests/test_conv_epilogue_cpu.py).
+// No wgmma / TMA in this header: tests/simt_cpu executes it from source on the CPU (tests/test_conv_epilogue_cpu.py).
 #pragma once
 #include "cd_common.cuh"
 

@@ -1,6 +1,6 @@
 // fp32 CUDA-core implementation of the tap-list convolution contract in colddiff.h.
 // Used (a) where channel counts are not tensor-core shaped (3-channel image edges), (b) as the
-// on-device fp32 cross-check of the tcgen05 path, (c) for the weight gradient until the tcgen05
+// on-device fp32 cross-check of the tensor-core path, (c) for the weight gradient until the tensor-core
 // wgrad lands.  64 pixels x 64 out-channels per CTA, 4x4 register tile per thread.
 #include "cd_common.cuh"
 
@@ -154,7 +154,7 @@ conv_smallc_kernel(const SimtParams p) {
 // opt-in (cd_conv_simt_set_preload): the register-tiled image-edge kernels run ONE block of 8 warps per SM (~185-227 registers per
 // thread), so nothing hides the memory latency of the staging loop below; with the switch on, the (at most three) receptive-field
 // entries a thread stages per 64-pixel chunk are all loaded before the first one is stored.  Same values in the same places.
-static int g_simt_preload = 1;   // validated on a B200 in round 2
+static int g_simt_preload = 1;
 __device__ __forceinline__ void stage_patches_preload(float* patch_f, int KP, long long q0, long long pend, const float* __restrict__ src,
                                                       int ld, int C, int H, int W, int Hg, int Wg, int sy, int sx, int ntaps,
                                                       const int* dyv, const int* dxv) {
@@ -561,7 +561,7 @@ static int launch_colsum(const float* x, int ld, long long rows, int C, float* o
     int G = 1; while (G < nq && G < 32) G <<= 1;
     // rows per block: at most 1024, but aim for >= 4 blocks per SM (8192 rows x 512 channels gave 32 blocks)
     const int xb = cd_cdiv(nq, G);
-    long long rpb = rows * xb / (148 * 4);
+    long long rpb = rows * xb / (cd_num_sms() * 4);
     if (rpb > 1024) rpb = 1024;
     if (rpb < 64) rpb = 64;
     dim3 g2(xb, cd_cdiv(rows, rpb));
@@ -692,7 +692,7 @@ static int conv_fwd_simt(const CdConvDesc* d, cudaStream_t st) {
                         (!d->aux || (d->aux_ld % 4 == 0 && (reinterpret_cast<uintptr_t>(d->aux) & 15) == 0));
     if (vec_ok) {
       const long long chunks = cd_cdiv(total, 64);
-      long long blocks = 148 * 2; if (blocks > chunks) blocks = chunks;
+      long long blocks = cd_num_sms() * 2; if (blocks > chunks) blocks = chunks;
       const int cpb = cd_cdiv(chunks, blocks);
       const int grid = cd_cdiv(chunks, cpb);
       const int KQ = cd_cdiv(c0.ntaps * c0.C, 4);
@@ -752,7 +752,7 @@ extern "C" int cd_conv_wgrad(const CdConvDesc* d, const float* dout, int dout_ld
   const bool pow2_cq = d->Cout >= 4 && ((d->Cout >> 2) & ((d->Cout >> 2) - 1)) == 0;
   if (c.C <= 4 && Ksm <= kSmallK && !c.w_per_batch && d->Cout % 4 == 0 && d->Cout <= 128 && pow2_cq &&
       dout_ld % 4 == 0 && (reinterpret_cast<uintptr_t>(dout) & 15) == 0 && total >= 1024 && total < (1ll << 31)) {
-    int blocks = 148 * 2; if (blocks > cd_cdiv(total, 256)) blocks = cd_cdiv(total, 256);
+    int blocks = cd_num_sms() * 2; if (blocks > cd_cdiv(total, 256)) blocks = cd_cdiv(total, 256);
     p.pix_per_split = cd_cdiv(total, blocks);
     const int grid = cd_cdiv(total, p.pix_per_split);
     const int KQ = cd_cdiv(Ksm, 4);
@@ -763,14 +763,14 @@ extern "C" int cd_conv_wgrad(const CdConvDesc* d, const float* dout, int dout_ld
     else wgrad_smallc4_kernel<9><<<grid, 256, 0, st>>>(p, wpre);
     CD_LAUNCH_CHECK();
   } else if (c.C <= 4 && c.ntaps * c.C <= kSmallK && !c.w_per_batch) {
-    int splits = cd_cdiv(total, 512); if (splits > 148 * 16) splits = 148 * 16; if (splits < 1) splits = 1;
+    int splits = cd_cdiv(total, 512); if (splits > cd_num_sms() * 16) splits = cd_num_sms() * 16; if (splits < 1) splits = 1;
     p.pix_per_split = cd_cdiv(total, splits);
     dim3 grid(cd_cdiv(total, p.pix_per_split), cd_cdiv(d->Cout, 128));
     wgrad_smallc_kernel<<<grid, 128, 0, st>>>(p);
     CD_LAUNCH_CHECK();
   } else {
   const int tiles = cd_cdiv(d->Cout, TM) * cd_cdiv(c.C, TNc) * c.ntaps;
-  int splits = cd_cdiv(148 * 4, tiles);
+  int splits = cd_cdiv(cd_num_sms() * 4, tiles);
   const int max_splits = cd_cdiv(total, 256);
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
@@ -822,7 +822,7 @@ extern "C" int cd_pack_weight(const float* w, int O, int I, int KH, int KW, int 
     CD_LAUNCH_CHECK();
     return 0;
   }
-  int blocks = cd_cdiv(total, 256); if (blocks > 148 * 8) blocks = 148 * 8;
+  int blocks = cd_cdiv(total, 256); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8;
   pack_weight_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(w, O, I, KH, KW, transposed_conv, mode,
                                                                           tl, ntaps, round_tf32, packed);
   CD_LAUNCH_CHECK();
@@ -842,7 +842,7 @@ extern "C" int cd_unpack_wgrad(const float* packed, int O, int I, int KH, int KW
     CD_LAUNCH_CHECK();
     return 0;
   }
-  int blocks = cd_cdiv(total, 256); if (blocks > 148 * 8) blocks = 148 * 8;
+  int blocks = cd_cdiv(total, 256); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8;
   unpack_wgrad_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(packed, O, I, KH, KW, transposed_conv,
                                                                             tl, ntaps, w_grad, accumulate);
   CD_LAUNCH_CHECK();

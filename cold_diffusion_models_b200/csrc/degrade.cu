@@ -214,7 +214,7 @@ __global__ void ema_kernel(float* __restrict__ ema, const float* __restrict__ p,
 }  // namespace
 
 extern "C" int cd_ema_update(float* ema, const float* p, int64_t n, float beta, int mode, void* stream) {
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > 148 * 16) blocks = 148 * 16; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 16) blocks = cd_num_sms() * 16; if (blocks < 1) blocks = 1;
   ema_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(ema, p, n, beta, mode);
   CD_LAUNCH_CHECK();
   return 0;
@@ -250,7 +250,7 @@ extern "C" int cd_blur_step_down(const float* xt, const float* xhat, float* out,
 extern "C" int cd_loss_fwd_bwd(const float* x0, const float* xhat, int64_t n, int mode, float grad_scale,
                                float* loss, float* dxhat, void* stream) {
   CD_REQUIRE(mode == 0 || mode == 1, "cd_loss_fwd_bwd: mode must be 0 (l1) or 1 (l2)");
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > 148 * 8) blocks = 148 * 8; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   loss_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x0, xhat, n, mode, 1.0f / static_cast<float>(n), grad_scale, loss, dxhat);
   CD_LAUNCH_CHECK();
   return 0;
@@ -263,7 +263,7 @@ extern "C" int cd_adam_ema_step(float* p, const float* g, float* m, float* v, fl
   // bias corrections in double on the host like torch.optim.Adam (1 - beta2^step loses ~5e-5 relative in fp32 at small steps)
   const float bc1 = static_cast<float>(1.0 - pow(static_cast<double>(beta1), static_cast<double>(step)));
   const float bc2s = static_cast<float>(sqrt(1.0 - pow(static_cast<double>(beta2), static_cast<double>(step))));
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > 148 * 16) blocks = 148 * 16; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 16) blocks = cd_num_sms() * 16; if (blocks < 1) blocks = 1;
   adam_ema_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(p, g, m, v, ema, n, lr, beta1, beta2, eps, bc1, bc2s,
                                                                        ema_mode, ema_beta, grad_scale);
   CD_LAUNCH_CHECK();
@@ -303,7 +303,7 @@ __global__ void noise_step_kernel(const float* __restrict__ img, const float* __
 
 extern "C" int cd_noise_lerp(const float* x1, const float* x2, const int64_t* t, int t_scalar, const float* sqrt_ac,
                              const float* sqrt_1mac, int64_t per_sample, int64_t n, float* out, void* stream) {
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > 148 * 8) blocks = 148 * 8; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   noise_lerp_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x1, x2, reinterpret_cast<const long long*>(t), t_scalar,
                                                                          sqrt_ac, sqrt_1mac, per_sample, n, out);
   CD_LAUNCH_CHECK();
@@ -313,7 +313,7 @@ extern "C" int cd_noise_lerp(const float* x1, const float* x2, const int64_t* t,
 extern "C" int cd_noise_step(const float* img, const float* x1_bar, const float* noise, int mode, int t, const float* sqrt_ac,
                              const float* sqrt_1mac, int64_t n, float* out, void* stream) {
   CD_REQUIRE(t >= 1 && (mode == 0 || (mode == 1 && noise)), "cd_noise_step: bad arguments");
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > 148 * 8) blocks = 148 * 8; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   noise_step_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(img, x1_bar, noise, mode, t, sqrt_ac, sqrt_1mac, n, out);
   CD_LAUNCH_CHECK();
   return 0;
@@ -355,7 +355,7 @@ __global__ void fade_step_kernel(const float* __restrict__ img, const float* __r
 extern "C" int cd_fade_lerp(const float* x1, const float* x2, const int64_t* t, int t_scalar, const float* alphas,
                             const float* one_minus_alphas, int B, int C, int HW, float* out, void* stream) {
   const long long n = static_cast<long long>(B) * C * HW;
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > 148 * 8) blocks = 148 * 8; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   fade_lerp_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x1, x2, reinterpret_cast<const long long*>(t), t_scalar,
                                                                         alphas, one_minus_alphas, C, HW, n, out);
   CD_LAUNCH_CHECK();
@@ -366,7 +366,7 @@ extern "C" int cd_fade_step(const float* img, const float* x1_bar, const float* 
                             const float* one_minus_alphas, int B, int C, int HW, float* out, void* stream) {
   CD_REQUIRE(t >= 1 && x2, "cd_fade_step: bad arguments");
   const long long n = static_cast<long long>(B) * C * HW;
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > 148 * 8) blocks = 148 * 8; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   fade_step_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(img, x1_bar, x2, t, alphas, one_minus_alphas, HW, n, out);
   CD_LAUNCH_CHECK();
   return 0;
@@ -421,7 +421,7 @@ __global__ void mask_step_down_kernel(const float* __restrict__ xt, const float*
 extern "C" int cd_mask_apply(const float* x, float* out, const float* masks, const int64_t* t, int t_scalar,
                              const int64_t* rx, const int64_t* ry, int B, int C, int S, int MS, int quantize, void* stream) {
   const long long n = static_cast<long long>(B) * C * S * S;
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > 148 * 8) blocks = 148 * 8; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   mask_apply_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, out, masks, reinterpret_cast<const long long*>(t), t_scalar,
       reinterpret_cast<const long long*>(rx), reinterpret_cast<const long long*>(ry), B, C, S, MS, quantize);
   CD_LAUNCH_CHECK();
@@ -431,7 +431,7 @@ extern "C" int cd_mask_apply(const float* x, float* out, const float* masks, con
 extern "C" int cd_mask_step_down(const float* xt, const float* xhat, float* out, const float* masks, int idx_hi, int idx_lo,
                                  const int64_t* rx, const int64_t* ry, int B, int C, int S, int MS, void* stream) {
   const long long n = static_cast<long long>(B) * C * S * S;
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > 148 * 8) blocks = 148 * 8; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   mask_step_down_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(xt, xhat, out, masks, idx_hi, idx_lo,
       reinterpret_cast<const long long*>(rx), reinterpret_cast<const long long*>(ry), B, C, S, MS);
   CD_LAUNCH_CHECK();
@@ -506,7 +506,7 @@ extern "C" int cd_chanmix(const float* xt, const float* xsrc, float* out, const 
                           const int64_t* t_lo, int hi_off, int lo_off, int B, int C, int64_t HW, int mode, void* stream) {
   CD_REQUIRE(C <= 8 && t_hi && (mode == 0 || (xt && t_lo)), "cd_chanmix: bad arguments");
   const long long n = static_cast<long long>(B) * HW;
-  int blocks = cd_cdiv(n, 256 * 2); if (blocks > 148 * 8) blocks = 148 * 8; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 2); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   chanmix_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(xt, xsrc, out, mats, reinterpret_cast<const long long*>(t_hi),
       reinterpret_cast<const long long*>(t_lo), hi_off, lo_off, B, C, HW, mode);
   CD_LAUNCH_CHECK();
@@ -518,7 +518,7 @@ extern "C" int cd_snow(const float* xt, const float* og, float* out, const float
                        int mode, void* stream) {
   CD_REQUIRE(t_hi && (mode == 0 || (xt && t_lo)), "cd_snow: bad arguments");
   const long long n = static_cast<long long>(B) * H * W;
-  int blocks = cd_cdiv(n, 256 * 2); if (blocks > 148 * 8) blocks = 148 * 8; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256 * 2); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   snow_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(xt, og, out, snow, br_coef, reinterpret_cast<const long long*>(t_hi),
       reinterpret_cast<const long long*>(t_lo), hi_off, lo_off, B, H, W, snow_batch, fix_brightness, mode);
   CD_LAUNCH_CHECK();

@@ -3,8 +3,7 @@
 // Same arithmetic, tile shapes and per-thread loops as dwconv7_pipe_kernel / dwconv7_wgrad_pipe_kernel (elementwise.cu; the
 // ConvNext depthwise convolution DB:145 and its backward).  Those kernels stage every (TY+6) x (TX+6) x 32-channel tile with
 // 16-byte LDGSTS: 13 copies per thread and item, each with its own row / column / bounds arithmetic -- ~490 of the ~3000
-// instructions a warp issues per item, in kernels that are instruction-issue bound (profiles/ncu_hbm_kernels_r02a.txt: issue
-// slots 70 % busy, which is what register-resident FFMA chains reach on this part: tools/micro/fma_rate.cu).  Here ONE thread
+// instructions a warp issues per item, in kernels that are instruction-issue bound.  Here ONE thread
 // issues ONE cp.async.bulk.tensor per tile: the 4-D box {32 channels, TX+6, TY+6, 1 image} lands densely in shared memory in
 // exactly the layout the LDGSTS version builds, the image border (zero padding of the convolution) is the tensor map's
 // out-of-bounds zero fill, and completion is an mbarrier the whole block waits on.

@@ -536,8 +536,8 @@ time_mlp_kernel(const long long* __restrict__ t, int dim, const float* __restric
 
 // conditioning rows of every ConvNextBlock (GELU -> Linear(dim, block_dim), DB:143-146) for all batch elements:
 // cond_all[b][o] = bc[o] + sum_i wc[o][i] * act(temb[b][i]), act = GELU (ConvNeXt Unet) or swish (DDPM Model, M2:121).
-// grid (row chunks, B); one warp per output row, lanes stride the (coalesced) weight row.  (Inside the one-block-per-sample
-// kernel above these ~6000 rows were 466 us of serial work.)
+// grid (row chunks, B); one warp per output row, lanes stride the (coalesced) weight row, so the ~6000 rows
+// are spread over the GPU instead of running serially inside the one-block-per-sample kernel above.
 constexpr int kCondRows = 64;
 __global__ void __launch_bounds__(256)
 cond_proj_kernel(const float* __restrict__ temb, int dim, const float* __restrict__ wc, const float* __restrict__ bc, int sumC,
@@ -1115,7 +1115,7 @@ extern "C" int cd_transpose_batched(const float* src, int ld, int B, int R, int 
 extern "C" int cd_upsample_nearest2x(const float* x, int x_ld, int B, int H, int W, int C, float* y, int y_ld, void* stream) {
   CD_REQUIRE(C % 4 == 0 && x_ld % 4 == 0 && y_ld % 4 == 0, "cd_upsample_nearest2x: C must be a multiple of 4");
   const long long total = static_cast<long long>(B) * 4 * H * W * (C / 4);
-  int blocks = cd_cdiv(total, 256); if (blocks > 148 * 16) blocks = 148 * 16;
+  int blocks = cd_cdiv(total, 256); if (blocks > cd_num_sms() * 16) blocks = cd_num_sms() * 16;
   upsample_nearest2x_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, x_ld, B, H, W, C, y, y_ld);
   CD_LAUNCH_CHECK();
   return 0;

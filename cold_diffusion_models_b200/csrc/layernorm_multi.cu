@@ -1,14 +1,13 @@
 // Channel LayerNorm forward for C <= 128 with PP pixels per lane group in flight (opt-in, cd_layernorm_set_multi).
 // layernorm_kernel<1> (elementwise.cu) gives every thread ONE float4 load before two shuffle reductions: 2048 resident threads x 16
-// bytes = 32 KB in flight per SM, about what HBM latency x bandwidth needs, and the kernel runs at 2.5 TB/s (23 launches, 0.5 ms of
-// a 9.2 ms reverse step).  Here a lane group loads PP pixels up front (PP x 16 bytes per thread in flight), then normalises them
+// bytes = 32 KB in flight per SM, about what HBM latency x bandwidth needs.  Here a lane group loads PP pixels up front (PP x 16 bytes per thread in flight), then normalises them
 // with the same per-pixel arithmetic in the same order (sum over the group by xor-shuffles, mean, centred sum of squares, rstd) --
 // bit-identical results.
 #include "cd_common.cuh"
 
 namespace {
 
-int g_ln_multi = 4;      // validated on a B200 in round 2 (bit-identical to the one-pixel kernel)
+int g_ln_multi = 4;
 
 template <int PP>
 __global__ void __launch_bounds__(256)

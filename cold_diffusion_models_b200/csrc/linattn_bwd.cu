@@ -4,8 +4,8 @@
 //   dv[n][e] = sum_d P[n][d] * dc[d][e]                         (dc = dctxn[b][h], 32 x 32 per head)
 //   dk[n][d] = P[n][d] * (sum_e v[n][e] * dc[d][e] - rowdot[d])
 //
-// Two [pixels x 32] x [32 x 32] products per head: on the CUDA cores they cost 4 shared-memory wavefronts per 32 FMAs and ran at
-// 0.3 of the HBM rate (515 us for the 128x128 level, profiles/op_profile_r02*.txt).  Here a warp owns 16 pixels of one head
+// Two [pixels x 32] x [32 x 32] products per head: on the CUDA cores they cost 4 shared-memory wavefronts per 32 FMAs and run far
+// below the HBM rate.  Here a warp owns 16 pixels of one head
 // and issues them as warp-level mma.sync.m16n8k8 TF32 in the 3xTF32 split (both operands hi + lo, three MMAs: fp32-grade
 // products -- the fp32 path of the engine keeps its 2e-6 gradient parity), accumulators in fp32.  k / v tiles of 32 pixels are double-buffered through shared memory with 16-byte
 // LDGSTS; dv and dk leave as 8-byte stores that fill whole 32-byte sectors.  No atomics: deterministic.

@@ -1,17 +1,16 @@
 // LinearAttention, the two per-(batch element, head) kernels with their operands STAGED through shared memory.
 // cd_linattn_weff and cd_linattn_bwd_small (elementwise.cu / backward.cu) run 4 x B blocks whose threads walk the `dim`
-// output channels with dependent strided global loads: 35 us and 100 us per call at a few MFLOP each (latency-bound; together
-// 2.2 ms of a 61 ms optimizer step and 0.3 ms of a 9.2 ms reverse step, profiles/op_profile_r01.txt).  The kernels below read
+// output channels with dependent strided global loads: a few MFLOP per call, bound by load latency.  The kernels below read
 // every operand once, 64 channel rows per pass with all loads of a pass in flight (one float4 per thread and array), and keep
 // the arithmetic ORDER of the originals (sums over co / d / e ascending, one fmaf per term), so their results are bit-identical
 // up to the order of the float atomics that were already there.
 // The same switch selects the bank-conflict-free thread mapping of attn_bwd_kv_kernel<REMAP> (backward.cu).
-// Off by default until they have run on a B200: cd_linattn_set_staged(1) / COLDDIFF_LINATTN_STAGED=1.
+// Switch: cd_linattn_set_staged(1) / COLDDIFF_LINATTN_STAGED=1.
 #include "cd_common.cuh"
 
 namespace {
 
-int g_staged = 1;        // validated on a B200 in round 2
+int g_staged = 1;
 constexpr int kRows = 64;            // channel rows (co) staged per pass
 
 // weff[b][co][h*32+d] = sum_e w_out[co][h*32+e] * ctxn[d][e],  ctxn[d][e] = ctx[b][h][d][e] * scale / ksum[b][h*32+d]

@@ -4,9 +4,7 @@
 // 295-299), the sinusoidal embedding (M2:6-24) and a small dense layer.  The dense convolutions and the batched matmuls of the
 // AttnBlock reuse cd_conv_fwd / cd_conv_wgrad (per-batch weights).
 //
-// STATUS (end of round 1): compiled and wired behind COLDDIFF_MODEL_TRAINING=1, not yet run on a B200 -- the GPU budget of the
-// round was spent before this file existed.  tests/test_model2_train_gpu.py (skipped unless that variable is set) checks every
-// parameter gradient against tests/golden/model2_grads_small.npz.
+// tests/test_model2_train_gpu.py checks every parameter gradient against tests/golden/model2_grads_small.npz.
 #include "cd_common.cuh"
 
 namespace {
@@ -221,7 +219,7 @@ extern "C" int cd_augment_u8(const uint8_t* src, int N, int Hs, int Ws, const in
                              const int32_t* flip, int B, int S, float* out, void* stream) {
   CD_REQUIRE(S <= Hs && S <= Ws && N >= 1 && B >= 1, "cd_augment_u8: crop %d does not fit the %dx%d source images", S, Hs, Ws);
   const long long n = static_cast<long long>(B) * S * S;
-  int blocks = cd_cdiv(n, 256); if (blocks > 148 * 16) blocks = 148 * 16;
+  int blocks = cd_cdiv(n, 256); if (blocks > cd_num_sms() * 16) blocks = cd_num_sms() * 16;
   augment_u8_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(src, Hs, Ws, reinterpret_cast<const long long*>(index), oy, ox, flip, B, S, out);
   CD_LAUNCH_CHECK();
   return 0;
@@ -242,7 +240,7 @@ extern "C" int cd_groupnorm_bwd(const float* x, int x_ld, int B, int64_t HW, int
 extern "C" int cd_dropout(const float* x, int x_ld, int64_t npix, int C, float p, uint64_t seed, float* y, int y_ld, void* stream) {
   CD_REQUIRE(p >= 0.f && p < 1.f, "cd_dropout: p must be in [0, 1)");
   const long long n = static_cast<long long>(npix) * C;
-  int blocks = cd_cdiv(n, 256); if (blocks > 148 * 16) blocks = 148 * 16; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(n, 256); if (blocks > cd_num_sms() * 16) blocks = cd_num_sms() * 16; if (blocks < 1) blocks = 1;
   dropout_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, x_ld, npix, C, p, seed, y, y_ld);
   CD_LAUNCH_CHECK();
   return 0;
@@ -257,7 +255,7 @@ extern "C" int cd_softmax_bwd_rows(const float* s, float* ds, int ld, int64_t ro
 extern "C" int cd_upsample_nearest2x_bwd(const float* dy, int dy_ld, int B, int H, int W, int C, float* dx, int dx_ld, void* stream) {
   CD_REQUIRE(C % 4 == 0 && dy_ld % 4 == 0 && dx_ld % 4 == 0, "cd_upsample_nearest2x_bwd: C must be a multiple of 4");
   const long long total = static_cast<long long>(B) * H * W * (C / 4);
-  int blocks = cd_cdiv(total, 256); if (blocks > 148 * 16) blocks = 148 * 16; if (blocks < 1) blocks = 1;
+  int blocks = cd_cdiv(total, 256); if (blocks > cd_num_sms() * 16) blocks = cd_num_sms() * 16; if (blocks < 1) blocks = 1;
   upsample_nearest2x_bwd_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(dy, dy_ld, B, H, W, C, dx, dx_ld);
   CD_LAUNCH_CHECK();
   return 0;

@@ -1,7 +1,7 @@
 // Batched weight repacks: every convolution weight of the network (reference layout OIHW / IOHW -> packed [tap][N][K]) and
 // every packed weight gradient (-> reference layout, accumulating) in ONE launch each.  The single-weight entry points
-// (cd_pack_weight / cd_unpack_wgrad, conv_simt.cu) cost one 10-15 us launch per weight: 64 + 98 launches, ~2 ms of a
-// 61 ms optimizer step (profiles/op_profile_r01.txt), for ~0.9 GB of traffic that is ~0.15 ms at HBM speed.
+// (cd_pack_weight / cd_unpack_wgrad, conv_simt.cu) cost one launch per weight: 64 + 98 latency-bound launches per optimizer
+// step for ~0.9 GB of traffic.
 // Here a block finds its job by a binary search over the ascending block0 column of a device-resident job table and
 // then does exactly what the single-weight kernels do for one tile.
 #include "cd_common.cuh"
@@ -134,7 +134,7 @@ unpack_wgrad_batched_kernel(const CdRepackJob* __restrict__ jobs, int njobs, int
 }
 
 // data-gradient operands straight from PACKED forward operands (the engine keeps dense conv weights packed [tap][O][I] as the
-// master copy: DESIGN.md section 3): dst[t][i][o] = src[tap_t][o][i] with tap_t = ky[t] * KW + kx[t].  One 32x32 transpose tile
+// master copy): dst[t][i][o] = src[tap_t][o][i] with tap_t = ky[t] * KW + kx[t].  One 32x32 transpose tile
 // per block through shared memory (both sides coalesced); job.nblocks = ntaps * ceil(O/32) * ceil(I/32).
 __global__ void __launch_bounds__(256)
 transpose_taps_batched_kernel(const CdRepackJob* __restrict__ jobs, int njobs) {

@@ -1,23 +1,24 @@
-// tcgen05 weight-gradient of the tap-list convolution (replaces cuDNN wgrad behind loss.backward() for the
+// Tensor-core weight gradient of the tap-list convolution (replaces cuDNN wgrad behind loss.backward() for the
 // dense convolutions of the reference Unet, DB:149-154,173-174,105-109):
 //
 //   dW[tap][co][ci] += sum_{pixels p} dY[p][co] * X[p (+) tap][ci]
 //
-// as a GEMM whose K dimension is the PIXEL axis: D[128 co x BN ci] (fp32, TMEM) += A^T B with both operands
-// "MN-major" in shared memory -- NHWC rows are exactly that: one 128-byte swizzled row per pixel holding 32
-// channels.  dY tiles ({32 co, CW px, R rows} TMA boxes) and X tiles land in SWIZZLE_128B smem and are
-// consumed by tcgen05.mma.kind::tf32 eight pixels (K = 8) at a time.  One CTA owns (co tile, ci tile, tap
-// group, pixel split) and keeps one TMEM accumulator per tap of its group (<= 4 x 128 columns); with
-// `halo` mode the dx = -1/0/+1 taps of a 3x3 kernel share ONE X tile that carries a one-pixel halo and are
-// addressed by shifting the descriptor start by whole 128-byte rows.  Partial sums of the pixel splits are
+// as a GEMM whose K dimension is the PIXEL axis.  NHWC rows hold the channels contiguously, i.e. both operands are
+// MN-major, which TF32 wgmma cannot read from shared memory; the MMAs are therefore mma.sync.m16n8k8 (TF32, fp32
+// accumulate) with their fragments read from the swizzled TMA tiles.  dY tiles ({32 co, CW px, R rows} TMA boxes) and
+// X tiles land in SWIZZLE_128B shared memory.  One CTA owns (co tile, ci tile, tap group, pixel split) and keeps one
+// register accumulator per tap of its group; with `halo` mode the dx = -1/0/+1 taps of a 3x3 kernel share ONE X tile
+// that carries a one-pixel halo and are addressed by shifting the pixel row.  Partial sums of the pixel splits are
 // combined with vector red.global.add.f32.
 #include "tc_common.cuh"
 
 namespace {
 
-constexpr int kThreads = 192;
+constexpr int kMmaWarps = 8;                      // 4 (co) x 2 (ci) warps, 32 co x BN/2 ci each
+constexpr int kThreads = 32 * (kMmaWarps + 1);    // + warp 8: TMA producer
 constexpr int kMaxTaps = 4;      // taps (accumulators) per CTA
 constexpr int kMaxGroups = 4;
+constexpr int kMaxAccCols = 256; // taps x BN: register accumulators of one CTA (128 co rows)
 
 struct WgParams {
   int B, Hg, Wg;
@@ -30,87 +31,56 @@ struct WgParams {
   int nloads[kMaxGroups];
   int tap_index[kMaxGroups][kMaxTaps];
   int tap_load[kMaxGroups][kMaxTaps];
-  int tap_shift[kMaxGroups][kMaxTaps];    // K-row shift inside the (halo) X tile
+  int tap_shift[kMaxGroups][kMaxTaps];    // pixel-row shift inside the (halo) X tile
   int load_dy[kMaxGroups][kMaxTaps], load_dx[kMaxGroups][kMaxTaps];
   int halo;                       // extra pixels per row in the X box (0 or 2)
   int sy, sx;                     // X coordinate = g*s + d
   int oys, oxs, oy0, ox0;         // dY coordinate = g*os + o0
-  int base_offset_mode;           // descriptor base_offset for row-shifted starts: 0 = none, 1 = (addr >> 7) & 7
   int per_batch, chunks_per_img, splits_per_img;   // per-batch weights: splits never cross images
   long long dw_batch_stride;
   float* dw;
   float* db;                      // BIAS kernels only: db[co] += sum over all pixels of dY (nullptr: not fused)
 };
 
-// MN-major operand for 32-bit (tf32) data: the only layout UMMA accepts is SWIZZLE_128B_BASE32B -- 128-byte rows (32
-// channels of one pixel), 32-byte swizzle atoms, pattern period 4 rows (512 B) -- which is what a TMA tensor map with
-// CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B writes.  32-channel chunks are `lbo` bytes apart, 4-pixel groups 512 B apart.
-__device__ __forceinline__ uint64_t make_mnmajor_sw128_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t base_off) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFFu);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>(512 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(base_off & 7u) << 49;
-  d |= static_cast<uint64_t>(1) << 61;                          // SWIZZLE_128B_BASE32B
-  return d;
+// element (row, c) of a 32-channel SWIZZLE_128B tile whose base is 1024-byte aligned: 16-byte chunk index XOR row % 8
+__device__ __forceinline__ float lds_sw(const uint8_t* base, int row, int c) {
+  return cd_round_tf32(*reinterpret_cast<const float*>(base + row * 128 + ((((c >> 2) ^ row) & 7) << 4) + (c & 3) * 4));
 }
-// same instruction without the "memory" clobber: volatile asm statements keep their order among themselves (barrier waits,
-// fences, commits), and ordinary loads of the constant descriptor table may then be scheduled across the MMAs
-__device__ __forceinline__ void mma_tf32_nomem(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n"
-               :: "r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(acc));
+__device__ __forceinline__ void mma_tf32_16x8x8(float (&d)[4], const float (&a)[4], const float (&b)[2]) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])),
+                 "r"(__float_as_uint(b[0])), "r"(__float_as_uint(b[1])));
 }
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" :: "l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" :: "l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 // BIAS = true (opt-in, cd_wgrad_tc_set_bias_fusion): the CTAs of the first ci tile and first tap group also accumulate the bias
-// gradient db[co] = sum_pixels dY[p][co] with one extra 128 x 32 x 8 MMA per k-step against a tile of ones (TMEM columns after
-// the tap accumulators), replacing the separate column-sum pass over dY.  BIAS = false is the production kernel.
-template <int BN, bool BIAS>
+// gradient db[co] = sum_pixels dY[p][co] from the dY fragments they load anyway, replacing the separate column-sum pass over dY.
+template <int BN, int NT, bool BIAS>
 __global__ void __launch_bounds__(kThreads, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_constant__ CUtensorMap mapX,
                 const WgParams p, int stages, int a_bytes, int b_bytes, int b_tx_bytes) {
   constexpr int NCH = BN / 32;                    // ci chunks of the B operand
-  // instruction descriptor: D=f32, A=B=tf32, A and B MN-major, N=BN, M=128
-  constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) |
-                              (uint32_t(BN >> 3) << 17) | (uint32_t(128 >> 4) << 24);
-  constexpr uint32_t kIdescBias = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) |
-                                  (uint32_t(32 >> 3) << 17) | (uint32_t(128 >> 4) << 24);
+  constexpr int NJ = BN / 16;                     // 8-wide n tiles per warp
+  static_assert(NT * BN <= kMaxAccCols, "accumulators of one CTA");
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint4 mma_tab[kMaxTaps * 8 + 8 + 1];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   const int g = blockIdx.z;
-  const int nl = p.nloads[g], nt = p.ntaps[g];
+  const int nl = p.nloads[g];
   const int stage_bytes = a_bytes + nl * b_bytes;
-  float* ones = reinterpret_cast<float*>(smem + stages * stage_bytes);          // BIAS: 8 pixels x 32 channels of 1.0f (1 KB)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + stages * stage_bytes + (BIAS ? 1024 : 0));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + stages * stage_bytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + stages;
-  uint64_t* done_bar = bars + 2 * stages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * stages + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr uint32_t kTmemCols = 512;
 
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(done_bar, 1);
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kMmaWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (BIAS) {
-    if (warp >= 2) for (int i = threadIdx.x - 64; i < 256; i += kThreads - 64) ones[i] = 1.f;
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> visible to the tensor-core (async) proxy
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int tile = blockIdx.x;
   const int co0 = (tile % p.tiles_co) * 128, ci0 = (tile / p.tiles_co) * BN;
@@ -126,10 +96,9 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_constant
     dw_off = n * p.dw_batch_stride;
   }
   const int nchunks = c_end > c_beg ? c_end - c_beg : 0;
-  const bool bias_cta = BIAS && p.db != nullptr && (tile / p.tiles_co) == 0 && g == 0;
 
-  if (warp == 0) {
-    // TMA producer: the whole warp walks the chunks and waits on the barriers, one elected lane issues (elect_one, tc_common.cuh)
+  if (warp == kMmaWarps) {
+    // TMA producer: the whole warp walks the chunks and waits on the barriers, one elected lane issues
     for (int it = 0; it < nchunks; ++it) {
       const int c = c_beg + it;
       const int cx = c % p.chunks_x;
@@ -153,108 +122,117 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_constant
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    // ---- MMA issuer.  The operand offsets of the MMAs of one chunk do not depend on the chunk: tabulate them once
-    // (one entry per MMA: A / B start offsets in 16-byte units, B descriptor high word, accumulator column, accumulate flag)
-    // so that the single issuing thread spends one LDS.128 + two adds per tcgen05.mma -- a 128x128x8 TF32 MMA lasts ~64 clk,
-    // a 128x64x8 one ~32 clk, and descriptor arithmetic in the loop was what bounded the issue rate.
-    const uint32_t a_lbo = a_bytes / 4, b_lbo = b_bytes / NCH;
-    const int ksteps_row = p.CW / 8;                // MMAs per image row of the chunk
-    const int per_tap = p.R * ksteps_row;
-    const int ntap_mma = nt * per_tap;              // <= kMaxTaps * 8
-    const int nmma = ntap_mma + (bias_cta ? per_tap : 0);
-    if (lane == 0) mma_tab[nmma] = make_uint4(0, 0, 0, 0);
-    if (bias_cta && lane < per_tap) {               // bias entries: same A rows, B = the ones tile (flag bit 17), columns after the taps
-      const int r = lane / ksteps_row, j = lane % ksteps_row;
-      mma_tab[ntap_mma + lane] = make_uint4(((r * p.CW + j * 8) * 128) >> 4, 0, 0,
-                                            static_cast<uint32_t>(nt * BN) | ((r | j) != 0 ? 0x10000u : 0u) | 0x20000u);
-    }
-    if (lane < ntap_mma) {
-      const int t = lane / per_tap, r = (lane % per_tap) / ksteps_row, j = lane % ksteps_row;
-      const uint32_t arow = r * p.CW + j * 8;
-      const uint32_t brow = r * (p.CW + p.halo) + j * 8 + p.tap_shift[g][t];
-      const uint32_t boffs = p.tap_load[g][t] * b_bytes + brow * 128;      // stage bases are 1024-byte aligned
-      const uint32_t bo = p.base_offset_mode == 1 ? ((boffs >> 7) & 7u) : (p.base_offset_mode == 2 ? ((boffs >> 7) & 3u) : 0u);
-      const uint64_t dbt = make_mnmajor_sw128_desc(0, b_lbo, bo);
-      mma_tab[lane] = make_uint4((arow * 128) >> 4, boffs >> 4, static_cast<uint32_t>(dbt >> 32),
-                                 static_cast<uint32_t>(t * BN) | ((r | j) != 0 ? 0x10000u : 0u));
+    return;
+  }
+
+  // ---- MMA warps: warp (wm, wn) owns co rows [32 wm, 32 wm + 32) and ci columns [BN/2 wn, BN/2 wn + BN/2) of every tap
+  const int wm = warp & 3, wn = warp >> 2;
+  const int gq = lane >> 2, tq = lane & 3;
+  const bool bias_cta = BIAS && p.db != nullptr && (tile / p.tiles_co) == 0 && g == 0 && wn == 0;
+  int tap_load[NT], tap_shift[NT];
+#pragma unroll
+  for (int t = 0; t < NT; ++t) { tap_load[t] = p.tap_load[g][t]; tap_shift[t] = p.tap_shift[g][t]; }
+  float acc[NT][2][NJ][4];
+#pragma unroll
+  for (int t = 0; t < NT; ++t)
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[t][i][j][e] = 0.f;
+  float bsum[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+  const int ksteps = p.KR / 8, cw_shift = __ffs(p.CW) - 1, rowlen = p.CW + p.halo;
+  for (int it = 0; it < nchunks; ++it) {
+    const uint32_t stage = it % stages, ph = (it / stages) & 1u;
+    mbar_wait(&full_bar[stage], ph);
+    const uint8_t* sA = smem + stage * stage_bytes + wm * (a_bytes / 4);      // this warp's 32 out-channels
+    const uint8_t* sB = smem + stage * stage_bytes + a_bytes;
+#pragma unroll 1
+    for (int ks = 0; ks < ksteps; ++ks) {
+      const int k0 = ks * 8 + tq, k1 = k0 + 4;          // pixels of this lane's A columns / B rows
+      float a[2][4];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        a[i][0] = lds_sw(sA, k0, i * 16 + gq);
+        a[i][1] = lds_sw(sA, k0, i * 16 + gq + 8);
+        a[i][2] = lds_sw(sA, k1, i * 16 + gq);
+        a[i][3] = lds_sw(sA, k1, i * 16 + gq + 8);
+        if (bias_cta) { bsum[i][0] += a[i][0] + a[i][2]; bsum[i][1] += a[i][1] + a[i][3]; }
+      }
+      const int r0 = (k0 >> cw_shift) * rowlen + (k0 & (p.CW - 1)), r1 = (k1 >> cw_shift) * rowlen + (k1 & (p.CW - 1));
+#pragma unroll
+      for (int t = 0; t < NT; ++t) {
+        const uint8_t* sBt = sB + tap_load[t] * b_bytes;
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+          const int cl = wn * (BN / 2) + j * 8 + gq;      // ci column (n) of this lane's B elements
+          const uint8_t* sBc = sBt + (cl >> 5) * (b_bytes / NCH);
+          const float b[2] = {lds_sw(sBc, r0 + tap_shift[t], cl & 31), lds_sw(sBc, r1 + tap_shift[t], cl & 31)};
+          mma_tf32_16x8x8(acc[t][0][j], a[0], b);
+          mma_tf32_16x8x8(acc[t][1][j], a[1], b);
+        }
+      }
     }
     __syncwarp();
-    {
-      const uint64_t da_t = make_mnmajor_sw128_desc(0, a_lbo, 0);
-      const uint32_t da_hi = static_cast<uint32_t>(da_t >> 32), da_lo = static_cast<uint32_t>(da_t);
-      const uint32_t db_lo = static_cast<uint32_t>(make_mnmajor_sw128_desc(0, b_lbo, 0));
-      const uint64_t ones_desc = make_mnmajor_sw128_desc(smem_u32(ones), 1024, 0);
-      for (int it = 0; it < nchunks; ++it) {
-        const uint32_t stage = it % stages, ph = (it / stages) & 1u;
-        mbar_wait(&full_bar[stage], ph);            // whole warp waits, one elected lane issues (elect_one, tc_common.cuh)
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sa16 = smem_u32(smem + stage * stage_bytes) >> 4;     // < 2^14: no carry into the LBO field
-          const uint32_t alo = da_lo + sa16, blo = db_lo + sa16 + (a_bytes >> 4);
-          const uint32_t first = it == 0 ? 0u : 0x10000u;
-          uint4 e = mma_tab[0];
-#pragma unroll 4
-          for (int i = 0; i < nmma; ++i) {
-            const uint4 en = mma_tab[i + 1];          // table has one spare entry; prefetched so the LDS latency is off the issue path
-            const uint64_t da = (static_cast<uint64_t>(da_hi) << 32) | (alo + e.x);
-            uint64_t db = (static_cast<uint64_t>(e.z) << 32) | (blo + e.y);
-            uint32_t idesc = kIdesc;
-            if (BIAS && (e.w & 0x20000u)) { db = ones_desc; idesc = kIdescBias; }
-            mma_tf32_nomem(tmem_base + (e.w & 0xFFFFu), da, db, idesc, (e.w | first) & 0x10000u);
-            e = en;
-          }
-          tc_commit(&empty_bar[stage]);
-        }
-        __syncwarp();
-      }
-      if (elect_one()) tc_commit(done_bar);
-      __syncwarp();
-    }
-  } else {
-    const int q = warp & 3;
-    const int co = co0 + q * 32 + lane;
-    mbar_wait(done_bar, 0);
-    tc_fence_after();
-    if (nchunks > 0) {
-      for (int t = 0; t < nt; ++t) {
-        float* wrow = p.dw + dw_off + (static_cast<long long>(p.tap_index[g][t]) * p.Cout + co) * p.Cin;
-#pragma unroll 1
-        for (int c = 0; c < BN; c += 32) {
-          uint32_t r[32];
-          tmem_ld32(tmem_base + t * BN + c + (static_cast<uint32_t>(q * 32) << 16), r);
-          if (co < p.Cout && ci0 + c < p.Cin) {
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);
+  }
+  if (nchunks == 0) return;
 #pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              red_add_v4(wrow + ci0 + c + j, __uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-          }
+  for (int t = 0; t < NT; ++t) {
+    if (t >= p.ntaps[g]) break;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int co = co0 + wm * 32 + i * 16 + gq + h * 8;
+        if (co >= p.Cout) continue;
+        float* wrow = p.dw + dw_off + (static_cast<long long>(p.tap_index[g][t]) * p.Cout + co) * p.Cin;
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+          const int ci = ci0 + wn * (BN / 2) + j * 8 + tq * 2;
+          if (ci < p.Cin) red_add_v2(wrow + ci, acc[t][i][j][2 * h], acc[t][i][j][2 * h + 1]);
         }
-      }
-      if (BIAS && bias_cta) {                       // every column of the bias accumulator holds the same sum: take column 0
-        uint32_t r[32];
-        tmem_ld32(tmem_base + nt * BN + (static_cast<uint32_t>(q * 32) << 16), r);
-        if (co < p.Cout) atomicAdd(p.db + co, __uint_as_float(r[0]));
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(kTmemCols) : "memory");
+  if (BIAS && bias_cta) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float v = bsum[i][h];
+        v += __shfl_xor_sync(0xffffffffu, v, 1);
+        v += __shfl_xor_sync(0xffffffffu, v, 2);
+        const int co = co0 + wm * 32 + i * 16 + gq + h * 8;
+        if (tq == 0 && co < p.Cout) atomicAdd(p.db + co, v);
+      }
   }
 }
 
 
-int g_wg_mode = 1;      // 0: one X tile per tap; 1 (default, verified on B200: profiles/wgrad_modes_r01.txt): dx taps share one halo
-                        // tile via row-shifted descriptor starts, base_offset 0; 2/3: probes with base_offset=(addr>>7)&7 / &3 (wrong)
+int g_wg_mode = 1;      // 0: one X tile per tap; otherwise (default) the dx taps of a 3x3 kernel share one halo tile
 int g_sms = 0;
+
+template <int BN, int NT>
+int launch_wg(bool bias, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& mapDY, const CUtensorMap& mapX,
+              const WgParams& p, int stages, int a_bytes, int b_bytes, int b_tx) {
+  if (bias) {
+    CD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<BN, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    wgrad_tc_kernel<BN, NT, true><<<grid, kThreads, smem, st>>>(mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
+  } else {
+    CD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<BN, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    wgrad_tc_kernel<BN, NT, false><<<grid, kThreads, smem, st>>>(mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
+  }
+  CD_LAUNCH_CHECK();
+  return 0;
+}
 
 }  // namespace
 
 extern "C" int cd_wgrad_tc_set_mode(int mode) { g_wg_mode = mode; return 0; }
 
-// opt-in: fold the bias gradient (column sums of dY) into the tcgen05 weight gradient.  Off by default: not yet run on a B200.
+// opt-in: fold the bias gradient (column sums of dY) into the tensor-core weight gradient.  Off by default.
 static int g_wg_bias_fusion = 0;
 extern "C" int cd_wgrad_tc_set_bias_fusion(int enable) { g_wg_bias_fusion = enable; return 0; }
 
@@ -300,14 +278,13 @@ int cd_conv_wgrad_tc(const CdConvDesc* d, const float* dout, int dout_ld, float*
   p.B = d->B; p.Hg = d->Hg; p.Wg = d->Wg; p.Cout = d->Cout; p.Cin = c.C;
   p.sy = d->sy; p.sx = d->sx; p.oys = d->oys; p.oxs = d->oxs; p.oy0 = d->oy0; p.ox0 = d->ox0;
   p.dw = dw;
-  const int BN = c.C >= 128 ? 128 : 64;
+  int BN = c.C >= 128 ? 128 : 64;
   // ---- tap groups ----
   const bool is3x3 = (c.ntaps == 9 && d->sy == 1 && d->sx == 1);
   bool shape3 = is3x3;
   if (is3x3) for (int t = 0; t < 9; ++t) if (c.dy[t] != t / 3 - 1 || c.dx[t] != t % 3 - 1) shape3 = false;
   const bool halo = shape3 && g_wg_mode != 0;
   p.halo = halo ? 2 : 0;
-  p.base_offset_mode = (g_wg_mode == 2) ? 1 : (g_wg_mode == 3 ? 2 : 0);
   if (halo) {
     p.ngroups = 3;
     for (int gk = 0; gk < 3; ++gk) {
@@ -328,9 +305,10 @@ int cd_conv_wgrad_tc(const CdConvDesc* d, const float* dout, int dout_ld, float*
     }
   }
   const int max_taps = p.ntaps[0], max_loads = p.nloads[0];
-  if (max_taps * BN > 512) return 1;
+  if (max_taps * BN > kMaxAccCols) BN = 64;                    // register accumulators: taps x BN <= 256 columns per CTA
+  if (max_taps * BN > kMaxAccCols) return 1;
   // ---- pixel chunking: KR K-rows per stage ----
-  int KR = (max_loads <= 1) ? 64 : 32;           // (KR = 32 everywhere measured 25 % slower: r01 bench_8)
+  int KR = (max_loads <= 1) ? 64 : 32;
   if (static_cast<long long>(d->Hg) * d->Wg < KR) KR = d->Hg * d->Wg;
   if (KR < 8) return 1;
   p.CW = d->Wg < KR ? d->Wg : KR;
@@ -341,8 +319,8 @@ int cd_conv_wgrad_tc(const CdConvDesc* d, const float* dout, int dout_ld, float*
   p.total_chunks = d->B * p.chunks_x * p.chunks_y;
   p.tiles_co = cd_cdiv(d->Cout, 128); p.tiles_ci = cd_cdiv(c.C, BN);
   const int tiles = p.tiles_co * p.tiles_ci;
-  // MMAs of one chunk: taps x KR/8 k-steps, 128 x BN x 8 each (~68 clk at BN = 128: 128 B/clk of shared-memory operand reads)
-  const double chunk_clk = double(max_taps) * (KR / 8) * (BN == 128 ? 68.0 : 40.0);
+  // MMAs of one chunk: taps x KR/8 k-steps, 128 x BN x 8 each; modelled at 1024 TF32 FLOP/clk per SM for mma.sync (not measured)
+  const double chunk_clk = double(max_taps) * (KR / 8) * (BN == 128 ? 256.0 : 128.0);
   int splits;
   if (c.w_per_batch) {
     const int cpi = p.chunks_x * p.chunks_y;
@@ -370,20 +348,20 @@ int cd_conv_wgrad_tc(const CdConvDesc* d, const float* dout, int dout_ld, float*
   const int stage_bytes = a_bytes + max_loads * b_bytes;
   int stages = (224 * 1024) / stage_bytes; if (stages > 6) stages = 6;   // 3 x 68 KB halo stages fit the 227 KB carve-out
   if (stages < 2) return 1;
-  // bias fusion: dense output grid, one weight set, room for 32 more TMEM columns after the tap accumulators
-  const bool fuse_bias = g_wg_bias_fusion && db != nullptr && !c.w_per_batch && d->oys == 1 && d->oxs == 1 && max_taps * BN + 32 <= 512;
+  // bias fusion: dense output grid, one weight set
+  const bool fuse_bias = g_wg_bias_fusion && db != nullptr && !c.w_per_batch && d->oys == 1 && d->oxs == 1;
   p.db = fuse_bias ? db : nullptr;
-  const size_t smem = size_t(stages) * stage_bytes + 1024 + 256 + (fuse_bias ? 1024 : 0);
+  const size_t smem = size_t(stages) * stage_bytes + 1024 + 256;
 
   CUtensorMap mapDY, mapX;
-  const CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_TFLOAT32;
+  const CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;   // operands are rounded to TF32 (RN) as they are read
   {
     cuuint64_t dims[4] = {(cuuint64_t)d->Cout, (cuuint64_t)d->Wo, (cuuint64_t)d->Ho, (cuuint64_t)d->B};
     cuuint64_t strides[3] = {(cuuint64_t)dout_ld * 4, (cuuint64_t)dout_ld * 4 * d->Wo, (cuuint64_t)dout_ld * 4 * d->Wo * d->Ho};
     cuuint32_t box[4] = {32, (cuuint32_t)(p.CW * d->oxs), (cuuint32_t)(p.R * d->oys), 1};
     cuuint32_t estr[4] = {1, (cuuint32_t)d->oxs, (cuuint32_t)d->oys, 1};
     CUresult r = enc(&mapDY, dt, 4, const_cast<float*>(dout), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(dY) failed: %d", (int)r);
   }
   {
@@ -392,26 +370,17 @@ int cd_conv_wgrad_tc(const CdConvDesc* d, const float* dout, int dout_ld, float*
     cuuint32_t box[4] = {32, (cuuint32_t)((p.CW + p.halo) * d->sx), (cuuint32_t)(p.R * d->sy), 1};
     cuuint32_t estr[4] = {1, (cuuint32_t)d->sx, (cuuint32_t)d->sy, 1};
     CUresult r = enc(&mapX, dt, 4, const_cast<float*>(c.src), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(X) failed: %d", (int)r);
   }
   dim3 grid(tiles, p.splits, p.ngroups);
-  if (fuse_bias) {
-    if (BN == 128) {
-      CD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      wgrad_tc_kernel<128, true><<<grid, kThreads, smem, st>>>(mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
-    } else {
-      CD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      wgrad_tc_kernel<64, true><<<grid, kThreads, smem, st>>>(mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
-    }
-    if (bias_done) *bias_done = 1;
-  } else if (BN == 128) {
-    CD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    wgrad_tc_kernel<128, false><<<grid, kThreads, smem, st>>>(mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
-  } else {
-    CD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    wgrad_tc_kernel<64, false><<<grid, kThreads, smem, st>>>(mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
-  }
-  CD_LAUNCH_CHECK();
-  return 0;
+  int rc;
+  if (BN == 128) rc = max_taps == 1 ? launch_wg<128, 1>(fuse_bias, grid, smem, st, mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx)
+                                    : launch_wg<128, 2>(fuse_bias, grid, smem, st, mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
+  else if (max_taps == 1) rc = launch_wg<64, 1>(fuse_bias, grid, smem, st, mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
+  else if (max_taps == 2) rc = launch_wg<64, 2>(fuse_bias, grid, smem, st, mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
+  else if (max_taps == 3) rc = launch_wg<64, 3>(fuse_bias, grid, smem, st, mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
+  else rc = launch_wg<64, 4>(fuse_bias, grid, smem, st, mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
+  if (rc == 0 && fuse_bias && bias_done) *bias_done = 1;
+  return rc;
 }

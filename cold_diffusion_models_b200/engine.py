@@ -1,4 +1,4 @@
-"""UnetEngine -- host-side schedule of the sm_100a kernels that execute the reference `Unet.forward`
+"""UnetEngine -- host-side schedule of the sm_90a kernels that execute the reference `Unet.forward`
 (DB:256-282) on NHWC fp32 activations.  Python here only sequences C-ABI calls (include/colddiff.h) on
 torch's current stream and owns device buffers; it performs no arithmetic.
 
@@ -29,7 +29,7 @@ _BATCHED_REPACK = None
 
 def batched_repack(enable=None):
     """switch of the one-launch weight repacks (ops.RepackBatch: cd_pack_weight_batched / cd_unpack_wgrad_batched).  Default
-    from COLDDIFF_BATCHED_REPACK (off until the kernels have run on a B200; NOTES.md 'code that has not run on a B200 yet')."""
+    from COLDDIFF_BATCHED_REPACK (off by default)."""
     global _BATCHED_REPACK
     if enable is not None:
         _BATCHED_REPACK = bool(enable)
@@ -111,7 +111,7 @@ class UnetEngine(_BackwardHolder):
         self.sumC = off
         self.cond_blocks = [b for b in self.blocks.values() if b.cond_off is not None]
         # dense nn.Conv2d weights (3x3 of the blocks, 4x4 stride-2 Downsample, every 1x1): their master copy can live PACKED
-        # [KH*KW][O][I] -- the forward operand of the tap-list convolution and the layout the tcgen05 weight gradient writes --
+        # [KH*KW][O][I] -- the forward operand of the tap-list convolution and the layout the tensor-core weight gradient writes --
         # with the nn.Parameter a permuted (O, I, KH, KW) view of it (flatten_params / _setup_grads in engine_bwd.py)
         self.dense_convs = {}
         for mn, mod in unet.named_modules():
@@ -264,7 +264,7 @@ class UnetEngine(_BackwardHolder):
 
     @staticmethod
     def _tc_geometry_ok(desc):
-        """the tcgen05 kernels tile the pixel grid with power-of-two boxes; other image sizes use the fp32 CUDA-core kernel"""
+        """the tensor-core kernels tile the pixel grid with power-of-two boxes; other image sizes use the fp32 CUDA-core kernel"""
         w, h = desc.Wg, desc.Hg
         pow2 = lambda v: v > 0 and (v & (v - 1)) == 0
         return (w % 128 == 0) if w >= 128 else (pow2(w) and pow2(h))
@@ -295,7 +295,7 @@ class UnetEngine(_BackwardHolder):
         uniq = bs.name if save is not None else tag
         # image-edge block (din = 1 / 3 image channels): its two convolutions over `din` channels run on the tensor cores with K
         # padded to 32 zero-filled channels (activations and packed weights) instead of the register-tiled CUDA-core kernels,
-        # which ran ~10x off their HBM bound (480 us forward / 367 us weight gradient per 128x128 micro-batch)
+        # which are far from their HBM bound at these channel counts
         edge = bs.din % 32 != 0 and xpad is not None
         ld_h = bs.din if bs.din % 4 == 0 else 4
         ld_in = self._pad32(bs.din) if edge else ld_h

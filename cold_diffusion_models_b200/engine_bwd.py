@@ -1,7 +1,7 @@
 """Backward schedule of UnetEngine (training step of GaussianDiffusion.p_losses, DB:963-975 + loss.backward()).
 
 Every gradient the reference obtains from torch autograd through Unet.forward (DB:256-282) is produced here by
-sm_100a kernels: data-gradients of the dense convolutions are tap-list convolutions with transposed/flipped
+sm_90a kernels: data-gradients of the dense convolutions are tap-list convolutions with transposed/flipped
 packed weights (cd_conv_fwd), weight-gradients are cd_conv_wgrad, and the HBM-bound pieces have dedicated
 kernels (backward.cu).  Parameter gradients are ACCUMULATED into reference-layout views of one flat fp32
 buffer (`engine.flat_grad`), which is what the optimizer / the NCCL all-reduce consume.
@@ -67,7 +67,7 @@ class BackwardMixin:
             off, k = self._offsets[n]
             sl = self.flat_grad[off:off + k]
             if n in self.dense_convs:
-                # gradients of dense Conv2d weights are STORED packed [KH*KW][O][I] (the tcgen05 weight gradient writes that
+                # gradients of dense Conv2d weights are STORED packed [KH*KW][O][I] (the tensor-core weight gradient writes that
                 # layout: no per-step unpack); .grad is the permuted reference-shaped view of the same memory
                 O, I, KH, KW = p.shape
                 self.G[n] = sl.view(KH, KW, O, I).permute(2, 3, 0, 1)

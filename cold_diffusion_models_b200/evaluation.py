@@ -1,4 +1,4 @@
-"""Evaluation path of the reference (SURVEY.md 8f rank 4): the metrics and figure / sample dumps its `*_test.py` drivers call
+"""Evaluation path of the reference: the metrics and figure / sample dumps its `*_test.py` drivers call
 on a trained model.  Everything here is host-side orchestration over the sampling methods of the diffusion classes (which
 run on the CUDA engine); the metrics themselves are small and, like in the reference, computed on the gathered CPU tensors.
 
@@ -7,7 +7,7 @@ Reference pieces this file stands in for:
     (deblurring_diffusion_pytorch.py:1160-1181, 1238-1722) -> `EvaluationMixin`
   * `Fid/fid_score.py:149-356` (activation statistics + Frechet distance) -> `get_activations`,
     `calculate_activation_statistics`, `calculate_frechet_distance`, `calculate_fid_given_samples`
-  * `pytorch_msssim.ssim` (third party, absent from /root/reference and from this image; restated from its published
+  * `pytorch_msssim.ssim` (third party, not part of the reference; restated from its published
     definition: 11-tap sigma-1.5 Gaussian window, 'valid' filtering, K = (0.01, 0.03)) -> `ssim`
   * `pycave.bayes.GaussianMixture` (third party, absent) -> `GaussianMixture` with the constructor / fit / sample surface the
     reference drivers use (celebA_128_test.py:129-138).  Only distributional agreement is possible there (EM from a random

@@ -1,13 +1,13 @@
 """`Model` -- the DDPM-style ResNet UNet of the reference (deblurring-diffusion-pytorch/deblurring_diffusion_pytorch/Model2.py
 :191-332, "M2"; used by the CIFAR-10 drivers, BASELINE config 2), with the reference's keyword-only constructor,
-`forward(x, t)` and state_dict keys, executed on the sm_100a engine (inference / sampling path).
+`forward(x, t)` and state_dict keys, executed on the sm_90a engine (inference / sampling path).
 
 Forward schedule (NHWC fp32): GroupNorm(32)+swish kernels (the time-embedding projection is folded into norm2's load),
-tcgen05 tap-list convolutions for conv1/conv2/nin_shortcut/q/k/v/proj_out/Downsample (asymmetric zero pad = TMA
+tensor-core tap-list convolutions for conv1/conv2/nin_shortcut/q/k/v/proj_out/Downsample (asymmetric zero pad = TMA
 out-of-bounds fill) and for the two batched matmuls of AttnBlock (per-batch-weight 1x1 convolutions: k is already
 the [n][C] weight slab, v is transposed once), a row-softmax kernel, and channel-sliced concat buffers instead of
 torch.cat.  Training (backward of GroupNorm / softmax attention, dropout) lives in model2_train.py and is reachable only
-with COLDDIFF_MODEL_TRAINING=1 until it has been validated on a B200; otherwise calling the model with autograd enabled raises.
+with COLDDIFF_MODEL_TRAINING=1 ; otherwise calling the model with autograd enabled raises.
 """
 import ctypes as C
 import torch
@@ -299,7 +299,7 @@ class Model(nn.Module):
     # ---------------------------------------------------------------------------------------------------------
     def forward(self, x, t):
         if not x.is_cuda:
-            raise RuntimeError("cold_diffusion_models_b200.Model runs on a B200 (CUDA) device only; got %s" % x.device)
+            raise RuntimeError("cold_diffusion_models_b200.Model runs on a CUDA device (H100) only; got %s" % x.device)
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             from . import model2_train
             return model2_train.ModelFunction.apply(self, x, t, *self.engine.param_list())

@@ -1,9 +1,9 @@
 """Training path of the DDPM-style `Model` (Model2.py:191-332, "M2"): forward that keeps what the backward needs, and the
-backward schedule, on the same sm_100a kernels as the ConvNeXt Unet (tap-list convolutions for every dense conv and for the
+backward schedule, on the same sm_90a kernels as the ConvNeXt Unet (tap-list convolutions for every dense conv and for the
 four batched matmuls of the AttnBlock backward; model2_bwd.cu for GroupNorm / softmax / upsample / dropout).
 
-STATUS: validated on a B200 in round 2 (profiles/gpu_tests_r02a.txt): tests/test_model2_train_gpu.py compares every parameter
-gradient with the reference (tests/golden/model2_grads_small.npz) on the fp32 and the tcgen05 path, checks the dropout mask
+STATUS: tests/test_model2_train_gpu.py compares every parameter
+gradient with the reference (tests/golden/model2_grads_small.npz) on the fp32 and the tensor-core path, checks the dropout mask
 consistency and one Trainer step.
 
 Gradient routing: every activation that the forward writes into a (slice of a) buffer has a gradient buffer of the same shape;

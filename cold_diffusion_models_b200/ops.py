@@ -66,7 +66,7 @@ class RepackBatch:
     normally once) and launches.  The block split mirrors the single-weight entry points: one block per 256 (o, i) rows
     for Conv2d weights with KH*KW <= 16, an element-strided range otherwise."""
 
-    MAX_STRIDED_BLOCKS = 148 * 2
+    MAX_STRIDED_BLOCKS = None       # cap on the blocks of an element-strided job; None: two per SM, as the single-weight entry points
 
     def __init__(self, kind):
         assert kind in ('pack', 'unpack')
@@ -105,7 +105,7 @@ class RepackBatch:
             if tiled:
                 nb = (O * I + 255) // 256
             else:
-                nb = min((len(taps) * O * I + 1023) // 1024, self.MAX_STRIDED_BLOCKS)
+                nb = min((len(taps) * O * I + 1023) // 1024, self.MAX_STRIDED_BLOCKS or 2 * sm_count(dst.device))
             r.block0, r.nblocks = b0, max(nb, 1)
             b0 += r.nblocks
         raw = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8)
@@ -236,17 +236,23 @@ def conv_wgrad(desc, dout, dw_packed, db=None, impl=CONV_SIMT):
 _SM_COUNT = {}
 
 
-def linattn_ctx_plan(B, n, device=None):
-    """how cd_linattn_context_det cuts the pixel axis of one image: -> (nblk, ppb) with ppb a multiple of 32 and
-    nblk = ceil(n / ppb) partials per image; about one wave of resident blocks (3 per SM) over the whole batch"""
+def sm_count(device=None):
+    """SM count of a CUDA device (132, the H100 SXM's, for CPU tensors and when there is no device): sizes the launch splits
+    that the host computes, like cd_num_sms() in the library"""
     key = str(device)
     sms = _SM_COUNT.get(key)
     if sms is None:
-        try:
-            sms = torch.cuda.get_device_properties(device).multi_processor_count if (device is not None and torch.device(device).type == 'cuda') else 148
-        except Exception:
-            sms = 148
+        sms = 132
+        if device is not None and torch.device(device).type == 'cuda' and torch.cuda.is_available():
+            sms = torch.cuda.get_device_properties(device).multi_processor_count
         _SM_COUNT[key] = sms
+    return sms
+
+
+def linattn_ctx_plan(B, n, device=None):
+    """how cd_linattn_context_det cuts the pixel axis of one image: -> (nblk, ppb) with ppb a multiple of 32 and
+    nblk = ceil(n / ppb) partials per image; about one wave of resident blocks (3 per SM) over the whole batch"""
+    sms = sm_count(device)
     per_img = max(1, (3 * sms) // max(B, 1))
     ppb = max(64, -(-(-(-n // per_img)) // 32) * 32)
     return -(-n // ppb), ppb

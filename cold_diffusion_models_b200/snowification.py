@@ -37,7 +37,7 @@ class DeColorization(ForwardProcessBase):
     def __init__(self, decolor_routine='Constant', decolor_ema_factor=0.9, decolor_total_remove=False, num_timesteps=50,
                  channels=3, to_lab=False):
         if to_lab:
-            raise NotImplementedError("to_lab (kornia Lab colour path) is out of scope of the B200 engine")
+            raise NotImplementedError("to_lab (kornia Lab colour path) is out of scope of the H100 engine")
         self.decolor_routine, self.decolor_ema_factor = decolor_routine, decolor_ema_factor
         self.decolor_total_remove, self.channels, self.num_timesteps = decolor_total_remove, channels, num_timesteps
         self.to_lab = to_lab
@@ -191,7 +191,7 @@ class GaussianDiffusion(nn.Module):
                                                   num_timesteps=self.num_timesteps, to_lab=to_lab)
         elif forward_process_type == 'Snow':
             if to_lab:
-                raise NotImplementedError("to_lab is out of scope of the B200 engine")
+                raise NotImplementedError("to_lab is out of scope of the H100 engine")
             self.forward_process = Snow(image_size=image_size, snow_level=snow_level, random_snow=random_snow,
                                         num_timesteps=self.num_timesteps, batch_size=batch_size, single_snow=single_snow,
                                         fix_brightness=fix_brightness)

@@ -1,4 +1,4 @@
-"""Drop-in `Trainer` for the *_diffusion_pytorch packages (reference: DB:1057-1236) on the B200 engine.
+"""Drop-in `Trainer` for the *_diffusion_pytorch packages (reference: DB:1057-1236) on the H100 engine.
 
 Same constructor keywords, attributes (`model`, `ema_model`, `opt`, `dl`, `ds`, `step`) and methods
 (`train`, `save`, `load`, `step_ema`, `reset_parameters`) and the same checkpoint format
@@ -74,10 +74,10 @@ class ImageFolderDataset(data.Dataset):
 
 class DeviceImageDataset:
     """The reference's Dataset / Dataset_Aug1 (DB:983-1026: Resize to 1.12 x S, then CenterCrop or RandomCrop + RandomHorizontalFlip,
-    ToTensor()*2-1) with the decoded, resized uint8 images resident in HBM: a 202k-image CelebA-128 set is 12.4 GB of the 180 GB.
+    ToTensor()*2-1) with the decoded, resized uint8 images resident in HBM: a 202k-image CelebA-128 set is 12.4 GB of the H100's 80 GB.
     Decoding and the one-time resize run once on the host (PIL, like the reference's transforms); every batch is one gather
     kernel (cd_augment_u8) with per-sample crop windows and flips drawn on the host -- no DataLoader workers, no H2D copy of
-    fp32 images.  Opt-in (`Trainer(..., dataset='device')` / `'device_aug'`); not yet run on a B200."""
+    fp32 images.  Opt-in (`Trainer(..., dataset='device')` / `'device_aug'`)."""
 
     def __init__(self, folder, image_size, augment=False, exts=('jpg', 'jpeg', 'png'), device='cuda', seed=0):
         import numpy as np
@@ -324,7 +324,7 @@ class Trainer(EvaluationMixin, object):
             u_loss = loss.detach() if u_loss is None else u_loss + loss.detach()
             if overlap and i == len(ds) - 1:
                 # last micro-batch: every finished suffix of the flat gradient is all-reduced while the backward continues
-                # (NCCL runs on its own stream behind the kernels enqueued so far; section 5 of DESIGN.md)
+                # (NCCL runs on its own stream behind the kernels enqueued so far)
                 def ready(lo, hi):
                     works.append(torch.distributed.all_reduce(eng.flat_grad[lo:hi], async_op=True))
                     low[0] = lo
@@ -530,7 +530,7 @@ class SnowificationTrainer(SnowEvaluationMixin, Trainer):
                  save_and_sample_every=5000, save_with_time_stamp_every=50000, results_folder='./results', load_path=None,
                  random_aug=False, torchvision_dataset=False, dataset=None, to_lab=False, order_seed=-1):
         if to_lab:
-            raise NotImplementedError("to_lab (kornia Lab colour path) is out of scope of the B200 engine")
+            raise NotImplementedError("to_lab (kornia Lab colour path) is out of scope of the H100 engine")
         core = _unwrap(diffusion_model)
         size = core.image_size
         self._size2 = tuple(size) if isinstance(size, (tuple, list)) else (size, size)

@@ -1,7 +1,7 @@
 """`Unet` -- the ConvNeXt restoration operator R(x, t) of the reference
 (deblurring-diffusion-pytorch/deblurring_diffusion_pytorch/deblurring_diffusion_pytorch.py:191-282, "DB"),
 with the reference's constructor, `forward(x, time)` signature and state_dict keys, executed by the
-sm_100a engine in engine.py (NHWC activations, tcgen05 tap-list convolutions, fused HBM kernels).
+sm_90a engine in engine.py (NHWC activations, tensor-core tap-list convolutions, fused HBM kernels).
 
 The nn.Module tree below only *holds parameters* under the reference's names (so reference checkpoints,
 including `module.`-prefixed DataParallel ones, load unchanged); no torch arithmetic runs on the hot path.
@@ -160,7 +160,7 @@ class Unet(nn.Module):
         `time` may be omitted only when the network was built with with_time_emb=False (snowification's UnetConvNextBlock
         declares `forward(x, time=None)`)."""
         if not x.is_cuda:
-            raise RuntimeError("cold_diffusion_models_b200.Unet runs on a B200 (CUDA) device only; got %s" % x.device)
+            raise RuntimeError("cold_diffusion_models_b200.Unet runs on a CUDA device (H100) only; got %s" % x.device)
         if time is None:
             if self.time_mlp is not None:
                 raise TypeError("Unet.forward: `time` is required when the network has a time embedding")

@@ -1,10 +1,10 @@
 /*
- * colddiff.h -- C ABI of libcolddiff.so: the B200 (sm_100a) engine behind the Cold-Diffusion
+ * colddiff.h -- C ABI of libcolddiff.so: the H100 (sm_90a) engine behind the Cold-Diffusion
  * hot path (GaussianDiffusion.p_losses training step + x0_step_down / ddim sampling around the
  * UNet restoration operator R(x,t) and the degradation operators D(x,t)).
  *
  * The upstream reference (arpitbansal297/Cold-Diffusion-Models) is pure Python/PyTorch and has NO
- * FFI / plugin interface of its own (SURVEY.md section 8b).  The boundary callers depend on is the
+ * FFI / plugin interface of its own.  The boundary callers depend on is the
  * Python class surface of each *_diffusion_pytorch package; cold_diffusion_models_b200/ mirrors
  * that surface and calls the entry points below through ctypes.  Every entry point cites the
  * reference code it replaces (DB = deblurring-diffusion-pytorch/deblurring_diffusion_pytorch/
@@ -47,7 +47,7 @@ int cd_last_error(char* buf, size_t n);
  *            src[s][b, gy*sy+dy[s][t], gx*sx+dx[s][t], ci] * w[s][(b*wb) , t, co, ci] )
  *   for (gy,gx) in the Hg x Wg GEMM pixel grid; reads outside the source image are zero.
  *
- * impl: CD_CONV_TC = tcgen05/TMA tensor-core kernel (kind::tf32, fp32 accumulate in TMEM;
+ * impl: CD_CONV_TC = wgmma/TMA tensor-core kernel (tf32, fp32 accumulate in registers;
  *       needs C[s] % 32 == 0 and 16-byte aligned rows), CD_CONV_SIMT = fp32 CUDA-core kernel
  *       (any shape; used for 3-channel image edges and as the on-device cross-check).
  * ------------------------------------------------------------------------------------------ */
@@ -104,7 +104,7 @@ int cd_unpack_wgrad(const float* packed, int O, int I, int KH, int KW, int trans
                     void* stream);
 
 /* The same two repacks for MANY weights in one launch (one optimizer step repacks ~64 convolution weights and
- * unpacks ~98 packed weight gradients: as single launches they are launch/latency-bound, ~2 ms of a 61 ms step).
+ * unpacks ~98 packed weight gradients: as single launches they are launch/latency-bound).
  * `jobs` is a DEVICE array of njobs descriptors (built once by the caller; pointers are stable across steps);
  * blocks [block0, block0 + nblocks) of the 256-thread grid of total_blocks work on job j, block0 ascending with j.
  * nblocks is the caller's choice (any value >= 1 is correct for transposed_conv / mode 1 / KH*KW > 16 jobs, which
@@ -189,50 +189,47 @@ int cd_conv1x1_to_nchw(const float* x, int ld, int B, int H, int W, int C, const
 int cd_nchw_to_nhwc(const float* x, int B, int C, int H, int W, float* out, int ld, void* stream);
 /* out[c] += sum_rows x[row*ld + c]  (bias / LayerNorm-beta gradients) */
 int cd_colsum(const float* x, int ld, int64_t rows, int C, float* out, void* stream);
-/* diagnostic switch for the tcgen05 wgrad: 0 = one X tile per tap, 1/2 = shared halo tile (base_offset 0 / computed) */
+/* diagnostic switch for the tensor-core wgrad: 0 = one X tile per tap, otherwise (default) the dx taps of a 3x3 kernel share one halo tile */
 int cd_wgrad_tc_set_mode(int mode);
-/* K-split policy of the tcgen05 wgrad: 0 = two waves rounded up, 1 / 2 = at most one / two full waves of CTAs,
+/* K-split policy of the tensor-core wgrad: 0 = two waves rounded up, 1 / 2 = at most one / two full waves of CTAs,
  * 3 (default) = minimise waves x (chunks_per_split x t_chunk + over_clk); over_clk > 0 sets the per-CTA fixed cost (SM clocks) */
 int cd_wgrad_tc_set_split(int policy, int over_clk);
-/* opt-in (default 0, not yet validated on a B200): fold the bias gradient (column sums of dY) into the tcgen05 weight gradient */
+/* opt-in (default 0): fold the bias gradient (column sums of dY) into the tensor-core weight gradient */
 int cd_wgrad_tc_set_bias_fusion(int enable);
 /* EXPERIMENTAL operand-format probe, not used by the engine (tools/conv_f16_probe.py): cd_conv_fwd with impl = CD_CONV_TC on FP16
  * operands -- d->s[i].src and d->s[i].w point to __half arrays (ld and the packed-weight layout count elements, C % 64 == 0),
- * tcgen05.mma.kind::f16 with fp32 accumulation, fp32 epilogue and outputs as usual. */
+ * wgmma on FP16 operands with fp32 accumulation, fp32 epilogue and outputs as usual. */
 int cd_conv_fwd_f16_probe(const CdConvDesc* d, void* stream);
-/* opt-in (default 0, not yet validated on a B200): line-coalesced epilogue of the tcgen05 convolution (csrc/conv_epilogue.cuh;
+/* opt-in (default 0): line-coalesced epilogue of the tensor-core convolution (csrc/conv_epilogue.cuh;
  * bit-identical results): 1 = for launches with at most 16 K chunks of 32 channels per tile (the store-bound 1x1 projections),
  * 2 = for every launch, 3 = at most 48 K chunks */
 int cd_conv_tc_set_staged_epilogue(int mode);
-/* opt-in (default 0, not yet validated on a B200): the register-tiled image-edge convolution / weight-gradient kernels (Cin <= 4)
+/* opt-in (default 0): the register-tiled image-edge convolution / weight-gradient kernels (Cin <= 4)
  * load all receptive-field entries of a 64-pixel chunk before storing the first (csrc/conv_simt.cu: stage_patches_preload), and
  * cd_conv1x1_to_nchw goes through a shared-memory tile (csrc/final_proj.cu), cd_conv1x1_to_nchw_bwd keeps four pixels per trip in
  * flight and cd_colsum_batched uses float4 loads (csrc/backward.cu): more bytes in flight, same arithmetic */
 int cd_conv_simt_set_preload(int enable);
-/* opt-in (default 0, not yet validated on a B200): channel LayerNorm forward for C <= 128 with 2 or 4 pixels per lane group in
+/* opt-in (default 0): channel LayerNorm forward for C <= 128 with 2 or 4 pixels per lane group in
  * flight (csrc/layernorm_multi.cu; same per-pixel arithmetic) */
 int cd_layernorm_set_multi(int pixels_per_group);
-/* opt-in (default 0, not yet validated on a B200): shared-memory-staged kernels behind cd_linattn_weff / cd_linattn_bwd_small
+/* opt-in (default 0): shared-memory-staged kernels behind cd_linattn_weff / cd_linattn_bwd_small
  * (csrc/linattn_small.cu; same arithmetic order as the default kernels) */
 int cd_linattn_set_staged(int enable);
-/* diagnostic switch: 1 (default) = TFLOAT32 tensor maps (TMA rounds fp32->tf32 RN on load) */
+/* diagnostic switch: 1 (default) = TFLOAT32 tensor maps, 0 = FLOAT32 tensor maps for the convolution operands */
 int cd_conv_tc_set_tf32_maps(int enable);
-/* SM-pair (tcgen05 cta_group::2, 256 pixels x 256 channels per pair) variant of the tap-list convolution:
- * 0 = off, 1 = where the tile cost model prefers it, 2 = wherever the problem is eligible (tests) */
+/* SM-pair variant of the tap-list convolution: a cluster of two CTAs computes two neighbouring 128-pixel tiles of the same output
+ * channels, each CTA fetching half of the weight tile and multicasting it to both.  0 = off (default), 1 = where the tile cost
+ * model prefers it (256-wide N tiles), 2 = wherever the problem is eligible (tests) */
 int cd_conv_tc_set_2cta(int mode);
-/* N tiles below 256 that also go to the SM-pair kernel (bit mask: 128 | 64; default 0): each CTA of the pair then stages 64 / 32
- * weight rows, which takes the shared-memory reads per MMA from 128 / 192 B/clk (one CTA) down to 96 / 160 B/clk */
+/* N tiles below 256 that also go to the SM-pair kernel (bit mask: 128 | 64; default 0) */
 int cd_conv_tc_set_2cta_bn(int mask);
-/* halo-tile kernel (csrc/conv_tc3.cu) for stride-1 convolutions whose taps lie in [-1, 1]^2 (dense 3x3 forward / data gradient,
- * fused [3x3 | 1x1] pairs): 128 GEMM rows = a 16 x 8 pixel patch whose 18 x 10 halo patch is fetched ONCE per channel chunk and
- * read by all nine taps through row-shifted shared-memory descriptors (6x less activation traffic from L2).  0 = off, 1 = on */
+/* halo-tile kernel for stride-1 convolutions whose taps lie in [-1, 1]^2 (dense 3x3 forward / data gradient, fused [3x3 | 1x1]
+ * pairs): the (16 + 2) x (TH + 2) halo patch of a 16 x TH pixel tile is fetched ONCE per 32-channel chunk and read by every tap.
+ * Bit mask: 1 = 16 x 8 tiles wherever eligible, 2 = 16 x 16 tiles (two accumulators per weight tile) for Cout <= 128 on grids of
+ * at least 32 x 32, 6 = 16 x 16 tiles wherever eligible (tests); 0 = off (default) */
 int cd_conv_tc_set_halo(int enable);
-/* timing experiments on the wide halo-tile kernel only (results are NOT written): 1 = epilogue without global accesses, 2 = without
- * TMEM loads either, 0 = normal */
-int cd_conv_tc_set_debug(int mode);
-/* two co-resident CTAs per SM (8 epilogue warps and half the pipeline stages each) for the one-CTA kernels with N <= 128: the single
- * MMA-issuing thread of a CTA is latency-bound (~8 clk per SASS instruction); two CTAs interleave two instruction streams on the
- * SM's tensor core.  Bit mask of N tiles (128 | 64); 0 = one CTA per SM */
+/* two co-resident CTAs per SM (half the pipeline stages each) for the tensor-core convolution with N <= 128: one CTA's epilogue
+ * overlaps the other's mainloop.  Bit mask of N tiles (128 | 64); default 192 (both), 0 = one CTA per SM */
 int cd_conv_tc_set_two_ctas(int mask);
 
 /* ------------------------------------------------------------------------------------------
@@ -253,7 +250,7 @@ int cd_linattn_bwd_small(const float* dweff, const float* ctx, const float* ksum
 int cd_linattn_bwd_kv(const float* qkv, int ld, int B, int n, const float* kmax, const float* ksum,
                       const float* dctxn, const float* rowdot, float* dqkv, int dld, void* stream);
 /* cd_linattn_bwd_kv runs its two [pixels x 32] x [32 x 32] products per head on warp-level tensor-core MMAs (csrc/linattn_bwd.cu:
- * 3xTF32: fp32-grade products); 0 selects the CUDA-core kernel of round 1 (A/B comparisons) */
+ * 3xTF32: fp32-grade products); 0 selects the CUDA-core kernel (A/B comparisons) */
 int cd_linattn_set_bwd_mma(int enable);
 int cd_transpose_weff(const float* weff, int B, int dim, float* weff_t, void* stream);
 int cd_conv1x1_to_nchw_bwd(const float* dout_nchw, const float* x, int ld, int B, int H, int W, int C,
@@ -382,7 +379,7 @@ int cd_linear_fwd(const float* x, int K, const float* w, const float* bias, int 
 
 /* Input pipeline (reference Dataset / Dataset_Aug1, DB:983-1026) with the decoded uint8 images resident in HBM ([N][Hs][Ws][3]):
  * out[b][c][y][x] = src[index[b]][oy[b]+y][ox[b] + (flip[b] ? S-1-x : x)][c] / 255 * 2 - 1   (RandomCrop / CenterCrop + flip + ToTensor*2-1).
- * Opt-in (Trainer(dataset='device...')); not yet run on a B200. */
+ * Opt-in (Trainer(dataset='device...')). */
 int cd_augment_u8(const uint8_t* src, int N, int Hs, int Ws, const int64_t* index, const int32_t* oy, const int32_t* ox,
                   const int32_t* flip, int B, int S, float* out, void* stream);
 

@@ -5,7 +5,7 @@ CPU fp32 restatement of the reference deblurring `GaussianDiffusion` hot path
 blur-kernel schedule (DB:348-389), q_sample (DB:927-960), p_losses (DB:963-975) and the
 Algorithm-1/2 sampling loop `sample` (DB:393-455) / `all_sample` (DB:609-689).
 
-The Gaussian taps come from torchgeometry (absent from /root/reference and from this
+The Gaussian taps come from torchgeometry (not part of the reference and absent from this
 image, un-pinned by the reference): restated in `gaussian_1d` from torchgeometry 0.1.2
 image/gaussian.py.  PARITY UNPINNED at that single boundary (<= last-ulp differences in
 <= 27 taps); everything else in this file is pinned against the real reference by

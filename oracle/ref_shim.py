@@ -2,17 +2,17 @@
 
 The reference packages import third-party modules that are absent from this
 image (comet_ml, torchgeometry, ...).  This module injects minimal stubs so the
-reference classes can be imported FROM /root/reference (never copied) and run on
+reference classes can be imported FROM a checkout of it ($COLD_REF_ROOT, never copied) and run on
 CPU to (a) generate golden vectors for tests/golden and (b) pin oracle/*.py.
 
 torchgeometry restatement (torchgeometry 0.1.2 image/gaussian.py, un-pinned by the
-reference; "parity unpinned" at this boundary, see DESIGN.md): gaussian(k, s)[x] =
+reference; "parity unpinned" at this boundary, see oracle/deblur_oracle.py): gaussian(k, s)[x] =
 exp(-(x - k//2)^2 / (2 s^2)) normalised to sum 1; 2-D kernel = outer product.
 """
 import sys, types, os, math
 import torch
 
-REF_ROOT = os.environ.get("COLD_REF_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("COLD_REF_ROOT", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "..", "reference"))
 
 
 def _gaussian(window_size, sigma):
@@ -90,7 +90,7 @@ def import_reference(pkg_dir, module):
                 setattr(sys.modules[modname], fn, lambda *a, **k: None)   # Lab colour path (--to_lab) is never exercised
     p = os.path.join(REF_ROOT, pkg_dir)
     if not os.path.isdir(p):
-        raise RuntimeError("reference not present at %s (only available in the build container)" % p)
+        raise RuntimeError("reference not present at %s (set $COLD_REF_ROOT to a checkout of the reference)" % p)
     # each reference directory defines same-named modules; purge before switching
     for k in list(sys.modules):
         if k.split(".")[0] == module:

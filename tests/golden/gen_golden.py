@@ -1,7 +1,8 @@
-"""Generate golden vectors FROM THE UNMODIFIED REFERENCE (run in the build container only;
-/root/reference does not exist on the GPU box).  Output: tests/golden/*.npz (committed).
+"""Generate golden vectors FROM THE UNMODIFIED REFERENCE (needs a checkout of the reference, found by oracle/ref_shim.py via
+$COLD_REF_ROOT).  Output: tests/golden/*.npz (committed).
 
-    python tests/golden/gen_golden.py
+    python tests/golden/gen_golden.py            # every golden of this script
+    python tests/golden/gen_golden.py config1    # config1_mnist_loss.npz only
 """
 import os, sys, io, contextlib
 import numpy as np
@@ -26,6 +27,29 @@ def save(name, **arrs):
         out[k] = v
     np.savez_compressed(os.path.join(HERE, name + '.npz'), **out)
     print('wrote', name, sum(np.asarray(v).nbytes for v in out.values()) // 1024, 'KiB')
+
+
+def gen_config1_mnist_loss():
+    """BASELINE config 1 (MNIST-shaped 1x32x32, T=20, k=11, sigma=7, Constant, B=4, full-size Unet): the reference's p_losses on
+    its Unet initialised under torch.manual_seed(0).  tests/test_oracle_golden.py rebuilds those weights with the package's Unet
+    under the same seed; that both draw identical parameters is asserted here."""
+    m = ref_shim.import_reference('deblurring-diffusion-pytorch', 'deblurring_diffusion_pytorch')
+    torch.manual_seed(0)
+    unet = quiet(m.Unet, dim=64, dim_mults=(1, 2, 4, 8), channels=1)
+    gd = m.GaussianDiffusion(unet, image_size=32, device_of_kernel='cpu', channels=1, timesteps=20,
+                             kernel_std=7.0, kernel_size=11, blur_routine='Constant', loss_type='l1')
+    torch.manual_seed(1234)
+    x = torch.rand(4, 1, 32, 32) * 2 - 1
+    t = torch.randint(0, 20, (4,))
+    with torch.no_grad():
+        ref_loss = gd.p_losses(x, t)
+    sys.path.insert(0, ROOT)
+    import cold_diffusion_models_b200 as cdm
+    torch.manual_seed(0)
+    ours = quiet(cdm.Unet, dim=64, dim_mults=(1, 2, 4, 8), channels=1).state_dict()
+    theirs = unet.state_dict()
+    assert set(ours) == set(theirs) and all(torch.equal(ours[k], theirs[k]) for k in theirs), "Unet initialisations differ"
+    save('config1_mnist_loss', x=x, t=t, ref_loss=np.float64(ref_loss.item()))
 
 
 def main():
@@ -224,4 +248,8 @@ def main():
 
 
 if __name__ == '__main__':
-    main()
+    if sys.argv[1:] == ['config1']:
+        gen_config1_mnist_loss()
+    else:
+        main()
+        gen_config1_mnist_loss()

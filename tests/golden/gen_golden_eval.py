@@ -1,4 +1,4 @@
-"""Goldens of the evaluation path from the UNMODIFIED reference (run in the build container, /root/reference present):
+"""Goldens of the evaluation path from the UNMODIFIED reference (needs a checkout of the reference):
 Frechet distances of `Fid/fid_score.py:calculate_frechet_distance` on seeded Gaussian statistics, including a rank-deficient
 pair (fewer observations than dimensions, the situation its eps-retry exists for), and `calculate_activation_statistics` with a
 stand-in feature network.  Usage: python tests/golden/gen_golden_eval.py   (deterministic)"""
@@ -8,7 +8,9 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-sys.path.insert(0, '/root/reference/deblurring-diffusion-pytorch')
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(HERE)), 'oracle'))
+import ref_shim  # noqa
+sys.path.insert(0, os.path.join(ref_shim.REF_ROOT, 'deblurring-diffusion-pytorch'))
 from Fid import fid_score  # noqa  (imports torchvision's inception definition; no weights are loaded)
 import scipy.linalg as _sl
 

@@ -1,6 +1,6 @@
 """Golden vectors FROM THE UNMODIFIED REFERENCE for the demixing and defading-generation packages and for the deblurring
-cover-figure trajectories (forward_and_backward / forward_and_backward_2).  Build container only (/root/reference is not on
-the GPU box).  Reuses the small Unet weights stored in unet_small.npz so the existing fixtures stay untouched.
+cover-figure trajectories (forward_and_backward / forward_and_backward_2).  Needs a checkout of the reference
+($COLD_REF_ROOT, see oracle/ref_shim.py).  Reuses the small Unet weights stored in unet_small.npz so the existing fixtures stay untouched.
 
     python tests/golden/gen_golden_more.py     ->  tests/golden/{demixing_small,defading_gen_small,fb_small}.npz
 """

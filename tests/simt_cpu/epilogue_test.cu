@@ -1,6 +1,6 @@
-// TEST INFRASTRUCTURE (never part of libcolddiff): drives cd_epilogue_staged32 of csrc/conv_epilogue.cuh the way the epilogue
-// warps of conv_tc_kernel do -- warp w of the block owns accumulator rows [32 w, 32 w + 32) of a 128 x BN tile, a lane holds the
-// 32 columns of one chunk of ITS row (what tcgen05.ld 32x32b.x32 returns), pixels map to arbitrary output rows.
+// TEST INFRASTRUCTURE (never part of libcolddiff): drives cd_epilogue_staged32 of csrc/conv_epilogue.cuh the way conv_tc_kernel
+// does after staging a warpgroup's accumulator chunk in shared memory -- warp w owns accumulator rows [32 w, 32 w + 32) of a
+// 128 x BN tile, a lane holds the 32 columns of one chunk of ITS row, pixels map to arbitrary output rows.
 #include "cd_common.cuh"
 #include "conv_epilogue.cuh"
 

@@ -1,8 +1,8 @@
 // TEST INFRASTRUCTURE: a minimal stand-in for <cuda_runtime.h> that lets the SIMT (CUDA-core) kernels of libcolddiff be
 // compiled by g++ and EXECUTED ON THE CPU, one thread block at a time, every CUDA thread a fiber (tests/simt_cpu/simt.cpp).
 // Barriers and warp shuffles are scheduling points; between two of them a thread runs alone, which is one of the legal
-// interleavings of a race-free kernel.  Not supported (the build script turns them into aborts): inline PTX, TMA, tcgen05.
-// Purpose: check indexing / reductions / launch geometry of kernels that have not run on a B200 yet.
+// interleavings of a race-free kernel.  Not supported (the build script turns them into aborts): inline PTX, TMA, wgmma.
+// Purpose: check indexing / reductions / launch geometry of the SIMT kernels without a GPU.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -70,7 +70,7 @@ static inline cudaError_t cudaMemsetAsync(void* p, int v, size_t n, cudaStream_t
 static inline cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t = nullptr) { memmove(d, s, n); return cudaSuccess; }
 static inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 static inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr a, int) {
-  *v = (a == cudaDevAttrMultiProcessorCount) ? 148 : 232448; return cudaSuccess; }
+  *v = (a == cudaDevAttrMultiProcessorCount) ? 132 : 232448; return cudaSuccess; }
 template <class F> static inline cudaError_t cudaFuncSetAttribute(F, cudaFuncAttribute, int) { return cudaSuccess; }
 int simt_occupancy();                                                    // settable from the test (default 2)
 template <class F> static inline cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int* n, F, int, size_t) {

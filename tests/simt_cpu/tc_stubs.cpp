@@ -1,4 +1,4 @@
-// TEST INFRASTRUCTURE: the tensor-core (tcgen05 / TMA) translation units cannot execute on the CPU.  In the all-SIMT CPU build
+// TEST INFRASTRUCTURE: the tensor-core (wgmma / TMA) translation units cannot execute on the CPU.  In the all-SIMT CPU build
 // of the library their internal entry points defer to the fp32 CUDA-core kernels of conv_simt.cu (the library's own fallback for
 // shapes that are not tensor-core shaped), and their tuning switches are accepted and ignored.
 #include "shim/cuda_runtime.h"
@@ -6,7 +6,6 @@
 
 extern "C" int cd_conv_fwd(const CdConvDesc* d, int impl, void* stream);
 int cd_conv_fwd_tc(const CdConvDesc* d, cudaStream_t st) { return cd_conv_fwd(d, CD_CONV_SIMT, st); }
-int cd_conv_fwd_tc2(const CdConvDesc*, cudaStream_t) { return 1; }
 int cd_conv_wgrad_tc(const CdConvDesc*, const float*, int, float*, float*, int* bias_done, cudaStream_t) { *bias_done = 0; return 1; }
 extern "C" int cd_conv_tc_set_tf32_maps(int) { return 0; }
 extern "C" int cd_conv_tc_set_2cta(int) { return 0; }
@@ -20,4 +19,3 @@ int cd_dwconv7_fwd_tma(const float*, int, int, int, int, int, const float*, cons
                        cudaStream_t) { return 1; }
 int cd_dwconv7_wgrad_tma(const float*, int, const float*, int, int, int, int, int, float*, cudaStream_t) { return 1; }
 extern "C" int cd_dwconv7_set_tma(int) { return 0; }
-extern "C" int cd_conv_tc_set_debug(int) { return 0; }

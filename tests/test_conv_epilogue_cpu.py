@@ -1,8 +1,7 @@
-"""The line-coalesced epilogue of the tcgen05 convolution (csrc/conv_epilogue.cuh, cd_conv_tc_set_staged_epilogue; opt-in, not
-yet run on a B200) executed from SOURCE on the CPU (tests/simt_cpu) inside a test kernel that feeds it like the epilogue warps of
+"""The line-coalesced epilogue of the tensor-core convolution (csrc/conv_epilogue.cuh, cd_conv_tc_set_staged_epilogue; opt-in) executed from SOURCE on the CPU (tests/simt_cpu) inside a test kernel that feeds it like the epilogue warps of
 conv_tc_kernel do, against a numpy statement of the row epilogue (acc + bias + resid -> out2 -> activation -> TF32 rounding -> out).
 Covers the transposition through the per-warp shared-memory tile, the pixel shuffles, invalid pixels, every optional operand,
-padded row strides and both thread orders.  The tcgen05 / TMA side of the kernel is not executable here: the `-m gpu` test is
+padded row strides and both thread orders.  The wgmma / TMA side of the kernel is not executable here: the `-m gpu` test is
 tests/test_helpers_and_variants_gpu.py::test_conv_staged_epilogue_matches_the_row_epilogue."""
 import ctypes as C
 import math

@@ -1,4 +1,4 @@
-"""GPU parity of the tap-list convolution (tcgen05 TC path and fp32 SIMT path) through the C ABI,
+"""GPU parity of the tap-list convolution (wgmma TC path and fp32 SIMT path) through the C ABI,
 against torch's fp64 CPU convolution on identical inputs."""
 import numpy as np
 import pytest
@@ -32,26 +32,27 @@ def ops():
 
 
 def run_conv(ops, d, impl):
-    """impl: 'simt' | 'tc' (1-CTA tcgen05) | 'tc2' (SM-pair cta_group::2 kernel where eligible, 256-wide tiles) | 'tc2n' (the
-    pair kernel also for the 128- and 64-wide N tiles)."""
+    """impl: 'simt' | 'tc' (one-CTA wgmma kernel) | 'tc2' (SM-pair two-CTA cluster kernel where eligible, 256-wide tiles) | 'tc2n'
+    (the pair kernel also for the 128- and 64-wide N tiles)."""
     from cold_diffusion_models_b200._lib import lib
     lib.cd_conv_tc_set_2cta(2 if impl in ('tc2', 'tc2n') else 0)
     lib.cd_conv_tc_set_2cta_bn(192 if impl == 'tc2n' else 0)
-    lib.cd_conv_tc_set_halo(1 if impl in ('tc3', 'tc3x2') else (6 if impl == 'tc4' else 0))   # 'tc3' / 'tc4': halo-tile kernels (csrc/conv_tc3.cu, conv_tc4.cu) where eligible
+    lib.cd_conv_tc_set_halo(1 if impl in ('tc3', 'tc3x2') else (6 if impl == 'tc4' else 0))   # 'tc3' / 'tc4': halo-tile kernel, 16 x 8 / 16 x 16 tiles, where eligible
     lib.cd_conv_tc_set_two_ctas(192 if impl in ('tcx2', 'tc3x2') else 0)  # '..x2': two CTAs per SM for the N <= 128 tiles
     try:
         ops.conv_fwd(d, ops.CONV_SIMT if impl == 'simt' else ops.CONV_TC)
         torch.cuda.synchronize()
     finally:
-        lib.cd_conv_tc_set_2cta(1)      # library default: pair kernel where the tile cost model prefers it
+        lib.cd_conv_tc_set_2cta(_DEFAULT_2CTA)
         lib.cd_conv_tc_set_2cta_bn(_DEFAULT_2CTA_BN)
         lib.cd_conv_tc_set_halo(_DEFAULT_HALO)
         lib.cd_conv_tc_set_two_ctas(_DEFAULT_TWO_CTAS)
 
 
-_DEFAULT_TWO_CTAS = 0           # library default of cd_conv_tc_set_two_ctas
-_DEFAULT_HALO = 2               # library default of cd_conv_tc_set_halo (wide halo-tile kernel where its tile count model says so)
-_DEFAULT_2CTA_BN = 128         # library default of cd_conv_tc_set_2cta_bn (narrow pair tiles)
+_DEFAULT_TWO_CTAS = 192         # library default of cd_conv_tc_set_two_ctas
+_DEFAULT_HALO = 0               # library default of cd_conv_tc_set_halo
+_DEFAULT_2CTA = 0               # library default of cd_conv_tc_set_2cta
+_DEFAULT_2CTA_BN = 0            # library default of cd_conv_tc_set_2cta_bn
 
 CASES = [
     # (B, Cin, Cout, H, W, k, pad)
@@ -122,8 +123,8 @@ def test_conv_two_sources_channel_slices(ops, impl):
 @pytest.mark.parametrize('case', [(2, 64, 64, 16, 8, 3), (1, 128, 128, 32, 24, 3), (3, 96, 320, 16, 16, 3), (2, 64, 64, 64, 64, 3),
                                   (1, 32, 64, 128, 128, 3), (2, 256, 256, 16, 16, 3)])
 def test_conv_halo_tile_kernel_forward_and_data_gradient(ops, case):
-    """csrc/conv_tc3.cu: one 18 x 10 halo patch per channel chunk read by all nine taps through row-shifted descriptors with a
-    1280-byte group stride -- forward taps, flipped (data-gradient) taps with the GELU' epilogue, single patch (16 x 8 image),
+    """halo-tile kernel, 16 x 8 tiles: one 18 x 10 halo patch per channel chunk read by all nine taps as shifted register
+    fragments -- forward taps, flipped (data-gradient) taps with the GELU' epilogue, single patch (16 x 8 image),
     non-square grids, Cout that is not a tile multiple, all three N tiles; against fp64 and against the per-tap kernel"""
     B, Ci, Co, H, W, k = case
     g = torch.Generator().manual_seed(sum(case))
@@ -162,8 +163,8 @@ def test_conv_halo_tile_kernel_forward_and_data_gradient(ops, case):
 @pytest.mark.parametrize('case', [(2, 64, 64, 16, 16, 3), (1, 128, 128, 32, 48, 3), (3, 96, 100, 16, 32, 3), (2, 128, 64, 64, 64, 3),
                                   (1, 32, 64, 128, 128, 3), (2, 256, 128, 32, 32, 3), (5, 64, 128, 16, 16, 3)])
 def test_conv_wide_halo_tile_kernel_forward_and_data_gradient(ops, case):
-    """csrc/conv_tc4.cu: one 18 x 18 halo patch per channel chunk, two 128-row blocks (left / right patch half, two TMEM accumulators)
-    per weight tile, 2304-byte group stride -- forward taps and flipped (data-gradient) taps with the GELU' epilogue, single patch,
+    """halo-tile kernel, 16 x 16 tiles: one 18 x 18 halo patch per channel chunk, two accumulators per consumer warpgroup that
+    share every weight tile -- forward taps and flipped (data-gradient) taps with the GELU' epilogue, single patch,
     non-square grids, Cout that is not a tile multiple, both N tiles, more tiles than SMs; against fp64 and the per-tap kernel"""
     B, Ci, Co, H, W, k = case
     g = torch.Generator().manual_seed(sum(case))
@@ -255,7 +256,7 @@ def test_conv_per_batch_weights(ops, impl):
 
 def test_tf32_operand_rounding_probe(ops):
     """Diagnostic (always passes): how does the TC path treat UNROUNDED fp32 operands under FLOAT32 vs
-    TFLOAT32 tensor maps?  Written to gpurun_out/tf32_probe.txt for DESIGN.md."""
+    TFLOAT32 tensor maps?  The errors are written next to the other test diagnostics."""
     import os
     from cold_diffusion_models_b200._lib import lib
     g = torch.Generator().manual_seed(21)
@@ -303,8 +304,8 @@ WG_CASES = [
 @pytest.mark.parametrize('mode', [0, 1, 2, 3])
 @pytest.mark.parametrize('case', WG_CASES)
 def test_wgrad_tc_matches_fp64(ops, case, mode):
-    """tcgen05 weight gradient (pixel-axis GEMM, MN-major operands) vs fp64; mode 0 = one X tile per tap,
-    1/2 = dx taps share one halo tile addressed by row-shifted descriptors (base_offset 0 / computed)."""
+    """tensor-core weight gradient (pixel-axis GEMM, MN-major operands) vs fp64; mode 0 = one X tile per tap,
+    otherwise the dx taps share one halo tile addressed by shifted pixel rows."""
     import os
     from cold_diffusion_models_b200._lib import lib
     B, Ci, Co, H, W, kind = case
@@ -359,8 +360,7 @@ def test_wgrad_tc_matches_fp64(ops, case, mode):
         os.makedirs('gpurun_out', exist_ok=True)
         with open('gpurun_out/wgrad_modes.txt', 'a') as f:
             f.write('mode %d case %s rel %.3e\n' % (mode, case, e))
-        if mode in (0, 1):   # modes 2-3 only probe the descriptor base_offset field and are expected to be wrong
-            assert e < 1e-5, e
+        assert e < 1e-5, e
     finally:
         lib.cd_wgrad_tc_set_mode(1)
 
@@ -384,7 +384,7 @@ def test_wgrad_per_batch(ops, impl, hw):
 
 @pytest.mark.parametrize('case', [(2, 64, 128, 32, 32, 3), (3, 128, 256, 16, 16, 3), (2, 64, 192, 32, 32, 1), (4, 256, 64, 16, 16, 3)])
 def test_wgrad_tc_fused_bias_gradient(ops, case):
-    """bias gradient folded into the tcgen05 weight gradient (one extra 128x32x8 MMA per k-step against a tile of ones):
+    """bias gradient folded into the tensor-core weight gradient (summed from the dY fragments the MMAs load):
     db and dW against fp64, and against the separate column-sum path"""
     from cold_diffusion_models_b200._lib import lib
     B, Ci, Co, H, W, k = case

@@ -3,7 +3,7 @@
 
 The host-logic suites (tests/test_*_host_logic.py) normally run on the numpy statement of the C ABI (tests/abi_emulator.py);
 with COLDDIFF_ABI_BACKEND=cuda_source the same tests run on the kernels themselves -- every SIMT kernel of the training step,
-the degradations, the reverse-process updates, the `Model` training kernels, the optimizer; the tcgen05 convolutions are replaced
+the degradations, the reverse-process updates, the `Model` training kernels, the optimizer; the tensor-core convolutions are replaced
 by the library's own fp32 CUDA-core convolution kernels.  All 28 host-logic tests pass that way (about 13 minutes):
 
     COLDDIFF_ABI_BACKEND=cuda_source python -m pytest tests/test_unet_host_logic.py tests/test_model2_host_logic.py \\

@@ -1,4 +1,4 @@
-"""Evaluation path (SURVEY.md 8f rank 4): metrics against the reference-generated goldens / the oracle, the mixture model
+"""Evaluation path: metrics against the reference-generated goldens / the oracle, the mixture model
 statistically, and the Trainer's evaluation methods end to end on CPU tensors through tests/abi_emulator.py (files written,
 index conventions, metric dictionary)."""
 import contextlib

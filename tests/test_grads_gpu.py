@@ -67,7 +67,7 @@ def test_unet_gradients_match_reference_golden_fp32_path():
 
 
 def test_unet_gradients_tf32_path_vs_oracle_autograd():
-    """tcgen05 (TF32) forward + data-gradient convolutions vs the fp32 CPU oracle's autograd, with the smooth L2 loss
+    """tensor-core (TF32) forward + data-gradient convolutions vs the fp32 CPU oracle's autograd, with the smooth L2 loss
     (the L1 loss' sign() gradient flips on 1e-4-level forward differences, which would mask what is being tested).
     The reference's own GPU path also runs convolutions in TF32 (torch.backends.cudnn.allow_tf32 defaults to True)."""
     import unet_oracle as UO
@@ -84,9 +84,7 @@ def test_unet_gradients_tf32_path_vs_oracle_autograd():
         f.write('median %.3e  p90 %.3e  max %.3e\n' % (errs[len(errs) // 2][0], errs[int(len(errs) * 0.9)][0], errs[-1][0]))
         for e, n in errs[-10:]:
             f.write('%.3e %s\n' % (e, n))
-    # measured on a B200: round 1 (profiles/grad_errors_tf32_r01.txt) median 9.6e-4, p90 1.19e-3, max 1.49e-3 per tensor; end of round 2
-    # (profiles/grad_errors_tf32_r02.txt) median 9.3e-4, p90 1.08e-3, max 1.35e-3 -- the TF32 operand
-    # rounding (2^-11 relative per operand, what cuDNN's default path does too) accumulated over the ~70 convolutions between the
+    # the TF32 operand rounding (2^-11 relative per operand, what cuDNN's default path does too) accumulated over the ~70 convolutions between the
     # loss and the first block; the fp32 CUDA-core path of the same schedule is at 2e-6 (test above)
     assert errs[len(errs) // 2][0] < 1.1e-3 and errs[-1][0] < 1.5e-3, errs[-3:]
 

@@ -1,7 +1,6 @@
 """GPU parity of the API helpers (Individual_Incremental, resolution Step routine / t = -1 rows, sample_from_blur, all_sample /
 forward_and_backward of every package, Unet constructor options, the evaluation routines) against the reference goldens, and of
-the kernel variants behind library switches against the kernels they replace (all validated on a B200 in round 2:
-profiles/gpu_tests_r02a.txt)."""
+the kernel variants behind library switches against the kernels they replace."""
 import io
 import contextlib
 import pytest
@@ -198,8 +197,7 @@ def test_evaluation_routines_on_the_gpu(unet, tmp_path, monkeypatch):
 
 @OPT_IN
 def test_batched_repack_matches_the_single_launches():
-    """csrc/repack.cu (one launch for all weight repacks / packed-gradient unpacks, COLDDIFF_BATCHED_REPACK; off by default until
-    this test has passed on a B200): bit-exact against the single-weight entry points on a job table that takes every branch,
+    """csrc/repack.cu (one launch for all weight repacks / packed-gradient unpacks, COLDDIFF_BATCHED_REPACK): bit-exact against the single-weight entry points on a job table that takes every branch,
     then the same Unet gradients with the switch on and off (float atomics in the weight-gradient kernels: TF32-level tolerance)"""
     from cold_diffusion_models_b200 import ops, engine
     from test_repack_batched import _job_set
@@ -248,8 +246,7 @@ def test_batched_repack_matches_the_single_launches():
 
 @OPT_IN
 def test_linattn_staged_kernels_match_the_default_ones():
-    """csrc/linattn_small.cu (cd_linattn_set_staged / COLDDIFF_LINATTN_STAGED; off by default until this test has passed on a
-    B200): same arithmetic order as the default kernels, so weff / dctxn / rowdot are bit-identical and dW_out (float atomics over
+    """csrc/linattn_small.cu (cd_linattn_set_staged / COLDDIFF_LINATTN_STAGED): same arithmetic order as the default kernels, so weff / dctxn / rowdot are bit-identical and dW_out (float atomics over
     the batch) agrees to rounding"""
     import ctypes as C
     from cold_diffusion_models_b200._lib import lib, ptr, stream, _check
@@ -307,7 +304,7 @@ def test_linattn_staged_kernels_match_the_default_ones():
 
 @OPT_IN
 def test_layernorm_multi_pixel_forward_matches_the_default_kernel():
-    """csrc/layernorm_multi.cu (cd_layernorm_set_multi; off by default until this test has passed on a B200): same per-pixel
+    """csrc/layernorm_multi.cu (cd_layernorm_set_multi): same per-pixel
     arithmetic as layernorm_kernel<1> -> bit-identical output and statistics"""
     import ctypes as C
     from cold_diffusion_models_b200._lib import lib, ptr, stream, _check
@@ -332,7 +329,7 @@ def test_layernorm_multi_pixel_forward_matches_the_default_kernel():
 
 @OPT_IN
 def test_image_edge_kernels_with_preloaded_staging_match_the_default():
-    """cd_conv_simt_set_preload (off by default until this test has passed on a B200): the 3-channel image-edge convolution and its
+    """cd_conv_simt_set_preload: the 3-channel image-edge convolution and its
     weight gradient with all receptive-field loads of a chunk in flight; outputs bit-identical, weight gradients (float atomics over
     blocks) to rounding"""
     from cold_diffusion_models_b200 import ops
@@ -410,8 +407,7 @@ def test_image_edge_kernels_with_preloaded_staging_match_the_default():
 
 @OPT_IN
 def test_conv_staged_epilogue_matches_the_row_epilogue():
-    """runs _conv_staged_epilogue_body in a child process with a time limit: the kernel variant it enables has never run on a
-    B200, and a tcgen05 / mbarrier pipeline that went wrong would spin instead of failing -- that must not take the session's
+    """runs _conv_staged_epilogue_body in a child process with a time limit: a wgmma / mbarrier pipeline that went wrong would spin instead of failing -- that must not take the session's
     CUDA context (and the tests after it) with it"""
     import os
     import subprocess
@@ -427,7 +423,7 @@ def test_conv_staged_epilogue_matches_the_row_epilogue():
 
 
 def _conv_staged_epilogue_body():
-    """csrc/conv_epilogue.cuh (cd_conv_tc_set_staged_epilogue; off by default until this test has passed on a B200): every tcgen05
+    """csrc/conv_epilogue.cuh (cd_conv_tc_set_staged_epilogue): every tensor-core
     convolution case of tests/test_conv_gpu.py again with the line-coalesced epilogue forced on all launches (mode 2: 3/4/6-stage
     kernels with the per-warp staging tiles), then bit-exact against the row epilogue on the store-bound 1x1 shapes in mode 1"""
     import test_conv_gpu as T
@@ -463,7 +459,7 @@ def _conv_staged_epilogue_body():
 @OPT_IN
 def test_fp16_operand_probe_agrees_with_the_tf32_kernel():
     """cd_conv_fwd_f16_probe (experimental, not used by the engine; tools/conv_f16_probe.py): kind::f16 MMAs on FP16 operands give
-    the TF32 kernel's result when both multiply the same (FP16-representable) values.  Child process with a time limit: tcgen05
+    the TF32 kernel's result when both multiply the same (FP16-representable) values.  Child process with a time limit: tensor-core
     code that has never run."""
     import os
     import subprocess

@@ -1,5 +1,5 @@
 """GPU parity of the `Model` (DDPM UNet) TRAINING path: every parameter gradient through the real library against the
-reference (tests/golden/model2_grads_small.npz), fp32 CUDA-core convolutions tight and tcgen05 (TF32) within the north-star
+reference (tests/golden/model2_grads_small.npz), fp32 CUDA-core convolutions tight and tensor-core (TF32) within the north-star
 tolerance, plus dropout consistency and one Trainer step.
 
 The host logic of the same schedule is checked on CPU by tests/test_model2_host_logic.py."""

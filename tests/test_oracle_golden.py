@@ -200,27 +200,22 @@ def test_model2_oracle_matches_reference():
     assert rel(xt, g['s_xt']) < 1e-5 and rel(dr, g['s_dr']) < 1e-5 and rel(img, g['s_img']) < 1e-4
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference only in build container')
 def test_oracle_matches_live_reference_config1_mnist():
-    """BASELINE config 1: MNIST-shaped 1x32x32, T=20, k=11, sigma=7, Constant, B=4, full-size Unet."""
-    import ref_shim, io, contextlib
-    m = ref_shim.import_reference('deblurring-diffusion-pytorch', 'deblurring_diffusion_pytorch')
+    """BASELINE config 1: MNIST-shaped 1x32x32, T=20, k=11, sigma=7, Constant, B=4, full-size Unet.  The reference's p_losses
+    on its Unet initialised under torch.manual_seed(0), with its inputs, is stored in tests/golden/config1_mnist_loss.npz; the
+    package's Unet draws the identical parameters under the same seed, so the full-size weights are rebuilt here."""
+    import io, contextlib
+    import cold_diffusion_models_b200 as cdm
+    g = load('config1_mnist_loss')
     torch.manual_seed(0)
     with contextlib.redirect_stdout(io.StringIO()):
-        unet = m.Unet(dim=64, dim_mults=(1, 2, 4, 8), channels=1)
-    gd = m.GaussianDiffusion(unet, image_size=32, device_of_kernel='cpu', channels=1, timesteps=20,
-                             kernel_std=7.0, kernel_size=11, blur_routine='Constant', loss_type='l1')
-    torch.manual_seed(1234)
-    x = torch.rand(4, 1, 32, 32) * 2 - 1
-    t = torch.randint(0, 20, (4,))
-    with torch.no_grad():
-        ref_loss = gd.p_losses(x, t)
+        unet = cdm.Unet(dim=64, dim_mults=(1, 2, 4, 8), channels=1)
     sd = unet.state_dict()
     o = DO.DeblurOracle(lambda a, b: UO.unet_forward(sd, a, b), image_size=32, channels=1, timesteps=20,
                         kernel_std=7.0, kernel_size=11, blur_routine='Constant')
     with torch.no_grad():
-        loss = o.p_losses(x, t)
-    assert abs(loss.item() - ref_loss.item()) < 1e-5
+        loss = o.p_losses(g['x'], g['t'])
+    assert abs(loss.item() - g['ref_loss'].item()) < 1e-5
 
 
 def _small_fn():

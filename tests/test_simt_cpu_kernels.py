@@ -1,8 +1,8 @@
-"""The CUDA SOURCE of SIMT kernels that have not run on a B200 yet, executed on the CPU (tests/simt_cpu: the .cu file is compiled
+"""The CUDA SOURCE of SIMT kernels that are off by default, executed on the CPU (tests/simt_cpu: the .cu file is compiled
 by g++ against a shim <cuda_runtime.h>, every CUDA thread is a fiber, barriers and warp shuffles are scheduling points) and
 compared with the numpy statement of the same entry point in tests/abi_emulator.py, which in turn is pinned to the reference
 goldens by tests/test_model2_host_logic.py.  Catches indexing, reduction and launch-geometry mistakes in the kernels themselves;
-says nothing about performance or about tcgen05 / TMA code (not executable this way)."""
+says nothing about performance or about wgmma / TMA code (not executable this way)."""
 import ctypes as C
 import ctypes as ctypes_mod
 import os

@@ -65,7 +65,7 @@ def test_gradients_follow_the_weights_across_fused_optimizer_steps(tmp_path):
     """the fused Adam kernel updates the flat parameter buffer through raw pointers (torch's version counters do not move): after
     every optimizer step BOTH pack generations (forward operands and the transposed data-gradient operands) must be rebuilt.
     Two optimizer steps at a large learning rate, then every parameter gradient at the NEW weights against the oracle's
-    autograd at the same weights (round 1 kept the step-0 data-gradient packs: several per cent off from step 2 on)."""
+    autograd at the same weights (stale data-gradient packs from step 0 would be several per cent off from step 2 on)."""
     import unet_oracle as UO
     import deblur_oracle as DO
     import cold_diffusion_models_b200 as cdm

@@ -271,7 +271,7 @@ def test_cuda_graph_replay_of_the_sampling_forward(small):
         finally:
             u.engine.enable_cuda_graph(False)
     for a, b in zip(eager, graphed):
-        assert torch.equal(a, b)          # same kernels on the same values: the forward is deterministic since round 2
+        assert torch.equal(a, b)          # same kernels on the same values: the forward is deterministic
 
 
 def test_all_sample_gen_sample_consistency(small):

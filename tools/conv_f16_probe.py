@@ -1,5 +1,5 @@
-"""Operand-format probe for round 2 (NOTES.md, "FP16 operands instead of TF32"): the tcgen05 tap-list convolution on FP16 sources and
-FP16 packed weights (cd_conv_fwd_f16_probe: kind::f16, fp32 accumulate, fp32 epilogue) next to today's TF32 kernel on the SAME
+"""Operand-format probe (FP16 operands instead of TF32): the tensor-core tap-list convolution on FP16 sources and
+FP16 packed weights (cd_conv_fwd_f16_probe: wgmma on FP16, fp32 accumulate, fp32 epilogue) next to today's TF32 kernel on the SAME
 values, for the convolution shapes of the config-3 network.  Inputs are rounded to FP16 first, which is also exactly representable
 in TF32 (both have a 10-bit mantissa), so the two kernels multiply identical numbers: outputs must agree to fp32 summation order.
 Prints per shape: TF32 us, FP16 us, TFLOP/s of both, max relative difference.
@@ -29,21 +29,17 @@ def run(B, H, Ci, Co, k, reps=5):
     out32, out16 = torch.empty(B, H, H, Co, device='cuda'), torch.empty(B, H, H, Co, device='cuda')
     d32 = ops.make_conv_desc([(ops.View(x32), taps, wp32, False)], ops.View(out32), (B, H, H), Cout=Co, bias=bias, act=ops.ACT_GELU)
     d16 = ops.make_conv_desc([(ops.View(x), taps, wp16, False)], ops.View(out16), (B, H, H), Cout=Co, bias=bias, act=ops.ACT_GELU)
-    lib.cd_conv_tc_set_2cta(0)
-    try:
-        t = []
-        for fn in (lambda: ops.conv_fwd(d32, ops.CONV_TC), lambda: _check(lib.cd_conv_fwd_f16_probe(C.byref(d16), stream()), 'cd_conv_fwd_f16_probe')):
-            fn(); fn()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            torch.cuda.synchronize()
-            e0.record()
-            for _ in range(reps):
-                fn()
-            e1.record()
-            torch.cuda.synchronize()
-            t.append(e0.elapsed_time(e1) / reps * 1e3)
-    finally:
-        lib.cd_conv_tc_set_2cta(1)
+    t = []
+    for fn in (lambda: ops.conv_fwd(d32, ops.CONV_TC), lambda: _check(lib.cd_conv_fwd_f16_probe(C.byref(d16), stream()), 'cd_conv_fwd_f16_probe')):
+        fn(); fn()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        t.append(e0.elapsed_time(e1) / reps * 1e3)
     err = ((out16.double() - out32.double()).norm() / out32.double().norm()).item()
     flops = 2.0 * B * H * H * Co * Ci * k * k
     return t[0], t[1], flops, err

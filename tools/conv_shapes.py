@@ -7,22 +7,21 @@ import cold_diffusion_models_b200 as cdm
 from cold_diffusion_models_b200._lib import lib
 
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 32
-# name: (2cta mode, 2cta N-tile mask, halo-kernel mask (1: conv_tc3, 2: conv_tc4), two-CTAs-per-SM mask)
+# name: (SM-pair mode, SM-pair N-tile mask, halo-kernel mask, two-CTAs-per-SM mask) -- cd_conv_tc_set_2cta / _2cta_bn / _halo /
+# _two_ctas
 CONFIGS = collections.OrderedDict([
-    ('1cta', (0, 0, 0, 0)),
-    ('pair256+128', (1, 128, 0, 0)),           # round-2 default before conv_tc4
-    ('wide-halo', (1, 128, 2, 0)),             # the default: conv_tc4 where its tile-count rule takes the layer
-    ('wide-halo-all', (1, 128, 6, 0)),         # conv_tc4 for every eligible layer
-    ('wh/noEpi', (1, 128, 2, 0, 1)),
-    ('wh/noStore', (1, 128, 2, 0, 3)),
-    ('wh/noGELU', (1, 128, 2, 0, 4)),
+    ('per-tap', (0, 0, 0, 0)),
+    ('pair256', (1, 0, 0, 0)),
+    ('pair+128', (1, 128, 0, 0)),
+    ('halo16x8', (0, 0, 1, 0)),
+    ('halo16x16', (0, 0, 2, 0)),
+    ('2ctas', (0, 0, 0, 192)),
 ])
-DEFAULT = (1, 128, 2, 0)
+DEFAULT = (0, 0, 0, 0)
 
 
 def apply(cfg):
     lib.cd_conv_tc_set_2cta(cfg[0]); lib.cd_conv_tc_set_2cta_bn(cfg[1]); lib.cd_conv_tc_set_halo(cfg[2]); lib.cd_conv_tc_set_two_ctas(cfg[3])
-    lib.cd_conv_tc_set_debug(cfg[4] if len(cfg) > 4 else 0)
 
 
 with contextlib.redirect_stdout(io.StringIO()):

@@ -30,7 +30,6 @@ def probe(tag, n=40):
 probe('default')
 lib.cd_dwconv7_set_pipe(0); probe('dwconv pipe off'); lib.cd_dwconv7_set_pipe(1)
 u.engine.conv_impl = CONV_SIMT; probe('conv SIMT'); u.engine.conv_impl = CONV_TC
-lib.cd_conv_tc_set_2cta(0); probe('2cta off'); lib.cd_conv_tc_set_2cta(1)
 # per-stage check: which engine buffers differ between two runs
 with torch.no_grad():
     u(x, t); torch.cuda.synchronize()

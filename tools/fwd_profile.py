@@ -1,5 +1,5 @@
 """One no_grad Unet forward (config 3 network, batch 32) between cudaProfilerStart/Stop after warm-up: the command behind the
-`ncu --profile-from-start off --set full -k regex:...` captures of the forward kernels in profiles/."""
+`ncu --profile-from-start off --set full -k regex:...` captures of the forward kernels."""
 import sys, io, contextlib, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

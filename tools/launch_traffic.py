@@ -1,6 +1,6 @@
 """`ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --csv` launch list of one optimizer step
-(tools/one_step.py) -> per-kernel table (launches, total us, DRAM MB, GB/s) and the DRAM bytes per launch of the tcgen05
-convolutions (profiles/conv_tc_traffic_rNN.json, what bench.py reports as roofline.traffic).
+(tools/one_step.py) -> per-kernel table (launches, total us, DRAM MB, GB/s) and the DRAM bytes per launch of the tensor-core
+convolutions.
 usage: launch_traffic.py launches.csv [out.json]"""
 import collections
 import csv

@@ -1,5 +1,5 @@
 """`ncu --page raw --csv` export -> a short per-launch table (duration, DRAM bytes and GB/s, L2 -> SM bytes, L2 hit rate,
-tensor-pipe / issue activity, registers, grid) for profiles/.  Usage: python tools/ncu_summary.py raw.csv [title] > summary.txt"""
+tensor-pipe / issue activity, registers, grid).  Usage: python tools/ncu_summary.py raw.csv [title] > summary.txt"""
 import csv
 import sys
 

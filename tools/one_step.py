@@ -1,5 +1,5 @@
 """One optimizer step of BASELINE config 3 (2 micro-batches of 32, 3x128x128, T=200) between cudaProfilerStart/Stop,
-after warm-up steps -- the command the ncu launch lists and full captures in profiles/ are taken from
+after warm-up steps, for profilers to capture
 (ncu --profile-from-start off ...)."""
 import sys, io, contextlib, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

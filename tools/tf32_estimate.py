@@ -1,7 +1,7 @@
 """CPU estimate of the TF32-path error of the multi-step GPU parity tests (tests/test_helpers_and_variants_gpu.py): runs the same
 calls on CPU tensors through tests/abi_emulator.py with both operands of every tensor-core convolution rounded to TF32 (RN,
 like the TFLOAT32 tensor maps), and prints the relative errors against the reference goldens.  Used to set tolerances before a
-test first runs on a B200.  Conservative: single forward of the small net 5.8e-4 here, 3e-4 measured on the GPU (DESIGN.md 3).  Usage: python tools/tf32_estimate.py"""
+test first runs on the GPU.  Conservative: single forward of the small net 5.8e-4 here.  Usage: python tools/tf32_estimate.py"""
 import os, sys, io, contextlib
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in ('', 'tests'):
@@ -9,7 +9,7 @@ for p in ('', 'tests'):
 import numpy as np, torch
 import abi_emulator
 abi_emulator.TF32_EMULATION = True
-if os.environ.get('COLDDIFF_OPERAND_FORMAT') == 'fp16':      # same estimate with FP16 operands (NOTES.md: FP16-operand option)
+if os.environ.get('COLDDIFF_OPERAND_FORMAT') == 'fp16':      # same estimate with FP16 operands
     abi_emulator._tf32 = lambda a: np.ascontiguousarray(a, dtype=np.float32).astype(np.float16).astype(np.float32)
 torch.Tensor.is_cuda = property(lambda self: True)
 torch.Tensor.cuda = lambda self, *a, **k: self
