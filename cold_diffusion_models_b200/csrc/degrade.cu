@@ -524,3 +524,120 @@ extern "C" int cd_snow(const float* xt, const float* og, float* out, const float
   CD_LAUNCH_CHECK();
   return 0;
 }
+
+// -------------------------------------------------------------------------------------------------------------
+// Lab colour path of the decolorization package (`to_lab=True`): rgb2lab / lab2rgb of diffusion/utils.py:113-222 ("UT")
+// and the decolorization step in Lab, rgb2lab(M_i lab2rgb(x)) (FP:189-195).  lab2rgb clamps fz and clips RGB to [0, 1]
+// at every step, so the steps do not compose into one matrix: every thread keeps its pixel's three values in registers
+// and runs the step chain 0..max(hi, lo), keeping the values after step hi and after step lo.
+// The sRGB <-> linear RGB and linear RGB <-> XYZ stages are kornia's (rgb_to_linear_rgb, linear_rgb_to_rgb, rgb_to_xyz,
+// xyz_to_rgb), which the reference imports without pinning a version; they are restated here from kornia's formulas, so
+// parity is unpinned at those constants.  Full-precision powf: the thresholds below select branches.
+// -------------------------------------------------------------------------------------------------------------
+namespace {
+__device__ __forceinline__ float srgb_to_linear(float x) {
+  return x > 0.04045f ? powf((x + 0.055f) / 1.055f, 2.4f) : x / 12.92f;
+}
+__device__ __forceinline__ float linear_to_srgb(float x) {
+  return x > 0.0031308f ? 1.055f * powf(fmaxf(x, 0.0031308f), 1.f / 2.4f) - 0.055f : 12.92f * x;
+}
+__device__ __forceinline__ float lab_f(float t) {          // UT:146-149
+  return t > 0.008856f ? powf(fmaxf(t, 0.008856f), 1.f / 3.f) : 7.787f * t + 4.f / 29.f;
+}
+__device__ __forceinline__ float lab_finv(float f) {       // UT:198-200
+  return f > 0.2068966f ? f * f * f : (f - 4.f / 29.f) / 7.787f;
+}
+// UT:113-163: RGB in [-1, 1] -> Lab (D65 white)
+__device__ __forceinline__ void rgb_to_lab(float r, float g, float b, float& L, float& A, float& Bb) {
+  r = srgb_to_linear((r + 1.f) * 0.5f); g = srgb_to_linear((g + 1.f) * 0.5f); b = srgb_to_linear((b + 1.f) * 0.5f);
+  const float x = 0.412453f * r + 0.357580f * g + 0.180423f * b;
+  const float y = 0.212671f * r + 0.715160f * g + 0.072169f * b;
+  const float z = 0.019334f * r + 0.119193f * g + 0.950227f * b;
+  const float fx = lab_f(x / 0.95047f), fy = lab_f(y), fz = lab_f(z / 1.08883f);
+  L = 116.f * fy - 16.f;
+  A = 500.f * (fx - fy);
+  Bb = 200.f * (fy - fz);
+}
+// UT:166-222: Lab -> 2 rgb - 1 (rgb clipped to [0, 1] when `clip`)
+__device__ __forceinline__ void lab_to_rgb(float L, float A, float Bb, bool clip, float& r, float& g, float& b) {
+  const float fy = (L + 16.f) / 116.f;
+  const float fx = A / 500.f + fy;
+  const float fz = fmaxf(fy - Bb / 200.f, 0.f);
+  const float x = lab_finv(fx) * 0.95047f, y = lab_finv(fy), z = lab_finv(fz) * 1.08883f;
+  r = linear_to_srgb(3.2404813432005266f * x + -1.5371515162713185f * y + -0.4985363261688878f * z);
+  g = linear_to_srgb(-0.9692549499965682f * x + 1.8759900014898907f * y + 0.0415559265582928f * z);
+  b = linear_to_srgb(0.0556466391351772f * x + -0.2040413383665112f * y + 1.0572251624579105f * z);
+  if (clip) { r = fminf(fmaxf(r, 0.f), 1.f); g = fminf(fmaxf(g, 0.f), 1.f); b = fminf(fmaxf(b, 0.f), 1.f); }
+  r = 2.f * r - 1.f; g = 2.f * g - 1.f; b = 2.f * b - 1.f;
+}
+
+__global__ void lab_convert_kernel(const float* x, float* out, int B, long long HW, int to_lab, int clip) {
+  // x and out may alias: every thread reads its pixel's three channels before writing them
+  const long long n = static_cast<long long>(B) * HW;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long b = i / HW, p = i % HW;
+    const long long o0 = b * 3 * HW + p, o1 = o0 + HW, o2 = o1 + HW;
+    const float v0 = x[o0], v1 = x[o1], v2 = x[o2];
+    float w0, w1, w2;
+    if (to_lab) rgb_to_lab(v0, v1, v2, w0, w1, w2);
+    else lab_to_rgb(v0, v1, v2, clip != 0, w0, w1, w2);
+    out[o0] = w0; out[o1] = w1; out[o2] = w2;
+  }
+}
+
+__global__ void chanmix_lab_kernel(const float* __restrict__ xt, const float* __restrict__ xsrc, float* __restrict__ out,
+                                   const float* __restrict__ mats, const long long* __restrict__ t_hi,
+                                   const long long* __restrict__ t_lo, int hi_off, int lo_off, int B, long long HW, int mode) {
+  // mode 0: out = D(xsrc, t_hi+hi_off) ; mode 1: out = xt - D(xsrc, t_hi+hi_off) + D(xsrc, t_lo+lo_off)
+  // D(v, k) = step k of ... step 0 of v, step i = rgb2lab(M_i lab2rgb(v)); index < 0 = v untouched
+  const long long n = static_cast<long long>(B) * HW;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int b = static_cast<int>(i / HW);
+    const long long p = i % HW;
+    const long long o0 = static_cast<long long>(b) * 3 * HW + p, o1 = o0 + HW, o2 = o1 + HW;
+    const int ih = static_cast<int>(t_hi[b]) + hi_off;
+    const int il = mode ? static_cast<int>(t_lo[b]) + lo_off : -1;
+    float c0 = xsrc[o0], c1 = xsrc[o1], c2 = xsrc[o2];
+    float h0 = c0, h1 = c1, h2 = c2, l0 = c0, l1 = c1, l2 = c2;
+    const int last = ih > il ? ih : il;
+    for (int s = 0; s <= last; ++s) {
+      float r, g, bl;
+      lab_to_rgb(c0, c1, c2, true, r, g, bl);
+      const float* M = mats + s * 9;
+      const float m0 = fmaf(__ldg(M + 2), bl, fmaf(__ldg(M + 1), g, __ldg(M + 0) * r));
+      const float m1 = fmaf(__ldg(M + 5), bl, fmaf(__ldg(M + 4), g, __ldg(M + 3) * r));
+      const float m2 = fmaf(__ldg(M + 8), bl, fmaf(__ldg(M + 7), g, __ldg(M + 6) * r));
+      rgb_to_lab(m0, m1, m2, c0, c1, c2);
+      if (s == ih) { h0 = c0; h1 = c1; h2 = c2; }
+      if (s == il) { l0 = c0; l1 = c1; l2 = c2; }
+    }
+    if (mode) {
+      out[o0] = xt[o0] - h0 + l0; out[o1] = xt[o1] - h1 + l1; out[o2] = xt[o2] - h2 + l2;
+    } else {
+      out[o0] = h0; out[o1] = h1; out[o2] = h2;
+    }
+  }
+}
+}  // namespace
+
+extern "C" int cd_lab_convert(const float* x, float* out, int B, int64_t HW, int to_lab, int clip, void* stream) {
+  CD_REQUIRE(x && out && B >= 0 && HW >= 0, "cd_lab_convert: bad arguments");
+  const long long n = static_cast<long long>(B) * HW;
+  if (n == 0) return 0;
+  int blocks = cd_cdiv(n, 256 * 2); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
+  lab_convert_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, out, B, HW, to_lab, clip);
+  CD_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int cd_chanmix_lab(const float* xt, const float* xsrc, float* out, const float* step_mats, const int64_t* t_hi,
+                              const int64_t* t_lo, int hi_off, int lo_off, int B, int64_t HW, int mode, void* stream) {
+  CD_REQUIRE(xsrc && out && step_mats && t_hi && (mode == 0 || (mode == 1 && xt && t_lo)), "cd_chanmix_lab: bad arguments");
+  const long long n = static_cast<long long>(B) * HW;
+  if (n == 0) return 0;
+  int blocks = cd_cdiv(n, 256 * 2); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
+  chanmix_lab_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(xt, xsrc, out, step_mats, reinterpret_cast<const long long*>(t_hi),
+      reinterpret_cast<const long long*>(t_lo), hi_off, lo_off, B, HW, mode);
+  CD_LAUNCH_CHECK();
+  return 0;
+}

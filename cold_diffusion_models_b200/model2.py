@@ -80,8 +80,11 @@ class AttnBlock(_P):
 
 class Model(nn.Module):
     def __init__(self, *, ch, out_ch, ch_mult=(1, 2, 4, 8), num_res_blocks, attn_resolutions, dropout=0.0,
-                 resamp_with_conv=True, in_channels, resolution):
+                 resamp_with_conv=True, in_channels, resolution, with_time_emb=True):
         super().__init__()
+        # with_time_emb=False (the snowification package's one-shot model, unet_resnet.py:291-301) keeps every time-embedding
+        # layer and runs them at t = 0 when forward() gets no t: same parameters, same checkpoints
+        self.with_time_emb = with_time_emb
         self.ch = ch
         self.temb_ch = self.ch * 4
         self.num_resolutions = len(ch_mult)
@@ -297,9 +300,13 @@ class Model(nn.Module):
         self._conv(ops.make_conv_desc([(View(ho), T1, P[name + '.proj_out'], False)], outv, (B, H, W), Cout=c, bias=a.proj_out.bias, resid=xv))
 
     # ---------------------------------------------------------------------------------------------------------
-    def forward(self, x, t):
+    def forward(self, x, t=None):
         if not x.is_cuda:
             raise RuntimeError("cold_diffusion_models_b200.Model runs on a CUDA device (H100) only; got %s" % x.device)
+        if t is None:
+            if getattr(self, 'with_time_emb', True):
+                raise ValueError("Model.forward needs t unless the model was built with with_time_emb=False")
+            t = torch.zeros(x.shape[0], dtype=torch.int64, device=x.device)
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             from . import model2_train
             return model2_train.ModelFunction.apply(self, x, t, *self.engine.param_list())

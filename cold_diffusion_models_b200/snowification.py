@@ -11,7 +11,11 @@ snowification/diffusion/diffusion.py:110-447 "SN", snowification/diffusion/forwa
 * per-sample masked stepping (`sample_one_step`, `sample_multi_step`, SN:195-256) and the `t == -1` pass-through rows
   of `q_sample` (SN:344-388) become per-sample indices handed to the kernels -- no Python loop over steps, no
   `torch.where` scatter per step.  `sample()` returns the reference's dict {'xt','direct_recons','recon'}.
-`to_lab=True` (kornia Lab colour path) is out of scope (SURVEY section 2.1) and raises.
+* `to_lab=True` (Lab colour path): the tensors the process sees hold Lab values.  A decolorization step is then
+  rgb2lab(M_i lab2rgb(x)) (FP:189-195), nonlinear because lab2rgb clamps and clips at every step, so D(x, t_b) runs the
+  per-step chain per pixel in registers (cd_chanmix_lab) instead of one cumulative matrix.  Snow takes no `to_lab`
+  upstream and applies its operator to whatever the tensor holds; for both processes `sample` / `all_sample` convert
+  their outputs back with lab2rgb (SN:287-290, 331-336).  `rgb2lab` / `lab2rgb` below are diffusion/utils.py's.
 """
 import ctypes as C
 import numpy as np
@@ -22,6 +26,30 @@ import torch.nn.functional as F
 from ._lib import call, ptr, stream
 from .deblurring import _LossFn
 from .degradation import gaussian_taps
+
+
+def _lab_convert(image, to_lab, clip=True):
+    if not torch.is_tensor(image):
+        raise TypeError(f"Input type is not a torch.Tensor. Got {type(image)}")
+    if image.dim() < 3 or image.shape[-3] != 3:
+        raise ValueError(f"Input size must have a shape of (*, 3, H, W). Got {image.shape}")
+    if not image.is_cuda:
+        raise RuntimeError("rgb2lab / lab2rgb run on a CUDA device (H100) only; got %s" % image.device)
+    x = image.contiguous().float()
+    out = torch.empty_like(x)
+    B = x.numel() // (3 * x.shape[-1] * x.shape[-2]) if x.numel() else 0
+    call('cd_lab_convert', ptr(x), ptr(out), B, C.c_int64(x.shape[-1] * x.shape[-2]), int(to_lab), int(bool(clip)), stream())
+    return out
+
+
+def rgb2lab(image):
+    """diffusion/utils.py:113-163: RGB in [-1, 1], shape (*, 3, H, W) -> Lab (L in 0..100), D65 white point"""
+    return _lab_convert(image, True)
+
+
+def lab2rgb(image, clip=True):
+    """diffusion/utils.py:166-222: Lab, shape (*, 3, H, W) -> RGB in [-1, 1] (2 rgb - 1; rgb clipped to [0, 1] when `clip`)"""
+    return _lab_convert(image, False, clip)
 
 
 class ForwardProcessBase:
@@ -36,8 +64,8 @@ class ForwardProcessBase:
 class DeColorization(ForwardProcessBase):
     def __init__(self, decolor_routine='Constant', decolor_ema_factor=0.9, decolor_total_remove=False, num_timesteps=50,
                  channels=3, to_lab=False):
-        if to_lab:
-            raise NotImplementedError("to_lab (kornia Lab colour path) is out of scope of the H100 engine")
+        if to_lab and channels != 3:
+            raise ValueError("to_lab needs 3-channel images, got channels=%d" % channels)
         self.decolor_routine, self.decolor_ema_factor = decolor_routine, decolor_ema_factor
         self.decolor_total_remove, self.channels, self.num_timesteps = decolor_total_remove, channels, num_timesteps
         self.to_lab = to_lab
@@ -51,6 +79,8 @@ class DeColorization(ForwardProcessBase):
             A = M.double().numpy() @ A
             cum.append(A.astype(np.float32))
         self.mats_cum = torch.from_numpy(np.stack(cum)) if cum else torch.zeros(0, Cn, Cn)
+        # the per-step table of the Lab path (cd_chanmix_lab): Lab steps do not compose into cumulative matrices
+        self.mats_step = torch.stack(self.step_mats).contiguous() if self.step_mats else torch.zeros(0, Cn, Cn)
 
     def get_factors(self):
         # FP:167-187
@@ -190,8 +220,7 @@ class GaussianDiffusion(nn.Module):
                                                   decolor_total_remove=decolor_total_remove, channels=channels,
                                                   num_timesteps=self.num_timesteps, to_lab=to_lab)
         elif forward_process_type == 'Snow':
-            if to_lab:
-                raise NotImplementedError("to_lab is out of scope of the H100 engine")
+            # the reference passes no `to_lab` to Snow: the snow operator acts on the tensor as it is (FP:361-372)
             self.forward_process = Snow(image_size=image_size, snow_level=snow_level, random_snow=random_snow,
                                         num_timesteps=self.num_timesteps, batch_size=batch_size, single_snow=single_snow,
                                         fix_brightness=fix_brightness)
@@ -202,11 +231,14 @@ class GaussianDiffusion(nn.Module):
         fp = self.forward_process
         if self._tables is None or self._tables[0] != dev or (isinstance(fp, Snow) and fp._dev is None):
             if isinstance(fp, DeColorization):
-                self._tables = (dev, fp.mats_cum.to(dev))
+                self._tables = (dev, (fp.mats_step if self._lab_decolor() else fp.mats_cum).to(dev))
             else:
                 self._tables = (dev, fp.layers(dev), fp.br_t.to(dev))
                 fp._dev = dev
         return self._tables
+
+    def _lab_decolor(self):
+        return self.to_lab and isinstance(self.forward_process, DeColorization)
 
     def _degrade(self, src, t_hi, hi_off, xt=None, t_lo=None, lo_off=0):
         """mode 0: D(src, t_hi+hi_off); mode 1 (xt given): xt - D(src, t_hi+hi_off) + D(src, t_lo+lo_off)"""
@@ -218,7 +250,10 @@ class GaussianDiffusion(nn.Module):
         t_hi = t_hi.to(device=src.device, dtype=torch.int64).contiguous()
         t_lo = t_lo.to(device=src.device, dtype=torch.int64).contiguous() if t_lo is not None else None
         xt = xt.contiguous() if xt is not None else None
-        if isinstance(self.forward_process, DeColorization):
+        if self._lab_decolor():
+            call('cd_chanmix_lab', ptr(xt), ptr(src), ptr(out), ptr(tab[1]), ptr(t_hi), ptr(t_lo), hi_off, lo_off, B,
+                 C.c_int64(H * W), mode, stream())
+        elif isinstance(self.forward_process, DeColorization):
             call('cd_chanmix', ptr(xt), ptr(src), ptr(out), ptr(tab[1]), ptr(t_hi), ptr(t_lo), hi_off, lo_off, B, Cc,
                  C.c_int64(H * W), mode, stream())
         else:
@@ -332,18 +367,25 @@ class GaussianDiffusion(nn.Module):
                 direct_recons = cur
             img = x
             t = t - 1
+        if self.to_lab:                                                             # SN:287-290
+            xt, direct_recons, img = lab2rgb(xt), lab2rgb(direct_recons), lab2rgb(img)
         return {'xt': xt, 'direct_recons': direct_recons, 'recon': img}
 
     def _total_forward(self, img):
-        """forward_process.total_forward: decolor = every channel <- channel mean (FP:198-218, independent of the schedule);
-        snow = D(img, T-1) (FP:358-359)"""
+        """forward_process.total_forward: decolor = every channel <- channel mean (FP:198-218, independent of the schedule),
+        in Lab mode rgb2lab(mean(lab2rgb(img))); snow = D(img, T-1) (FP:358-359)"""
         if isinstance(self.forward_process, DeColorization):
             img = img.contiguous().float()
             B, Cc, H, W = img.shape
             mat = torch.full((1, Cc, Cc), 1.0 / Cc, device=img.device, dtype=torch.float32)
             zero = torch.zeros(B, dtype=torch.int64, device=img.device)
             out = torch.empty_like(img)
-            call('cd_chanmix', ptr(None), ptr(img), ptr(out), ptr(mat), ptr(zero), ptr(None), 0, 0, B, Cc, C.c_int64(H * W), 0, stream())
+            if self.to_lab:                      # a one-step chain with the mean matrix
+                call('cd_chanmix_lab', ptr(None), ptr(img), ptr(out), ptr(mat), ptr(zero), ptr(None), 0, 0, B, C.c_int64(H * W), 0,
+                     stream())
+            else:
+                call('cd_chanmix', ptr(None), ptr(img), ptr(out), ptr(mat), ptr(zero), ptr(None), 0, 0, B, Cc, C.c_int64(H * W), 0,
+                     stream())
             return out
         tt = torch.full((img.shape[0],), self.num_timesteps, dtype=torch.long, device=img.device)
         return self._degrade(img, tt, -1)
@@ -362,8 +404,12 @@ class GaussianDiffusion(nn.Module):
         while times:
             step = torch.full((img.shape[0],), times - 1, dtype=torch.long, device=img.device)
             img, direct_recons = self.sample_one_step(img, step)
-            X_0s.append(direct_recons.cpu())
-            X_ts.append(img.cpu())
+            if self.to_lab:                      # SN:331-336 converts the CPU copies; same values, converted on the device
+                X_0s.append(lab2rgb(direct_recons).cpu())
+                X_ts.append(lab2rgb(img).cpu())
+            else:
+                X_0s.append(direct_recons.cpu())
+                X_ts.append(img.cpu())
             times = times - 1
         return X_0s, X_ts, None, []
 

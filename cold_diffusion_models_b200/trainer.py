@@ -523,14 +523,21 @@ def get_dataset(name, folder, image_size, random_aug=False):
 
 class SnowificationTrainer(SnowEvaluationMixin, Trainer):
     """Trainer of snowification/diffusion (== decolor-diffusion/diffusion), SN:563-760: the image size comes from the model,
-    torchvision datasets by name, `sample()` returns a dict whose entries are all saved, `save(save_with_time_stamp)`."""
+    torchvision datasets by name, `sample()` returns a dict whose entries are all saved, `save(save_with_time_stamp)`.
+
+    `to_lab=True`: every batch the reference passes through `post_process_func` (SN:613-625, 647: the cycled loader and
+    `_process_item`) is converted with rgb2lab, here on the device after the copy there (`post_process_func`): the training
+    batches (`_loss`, with or without `train_step(batches=)`), the periodic sample's start image and the evaluation batches
+    (`_eval_batch`, `_process_item`).  `train()` saves `og` after lab2rgb (SN:744-745).  Where the reference does not
+    convert, neither does this class:
+      * `fid_distance_decrease_from_manifold` reads `self.ds` directly, so its images stay RGB;
+      * `test_from_data` / `test_with_mixup` / `test_from_random` save the Lab start images as they are (`og` grids);
+      * `paper_invert_section_images` shows the Lab original next to the converted trajectories."""
 
     def __init__(self, diffusion_model, folder, *, ema_decay=0.995, image_size=128, train_batch_size=32, train_lr=2e-5,
                  train_num_steps=100000, gradient_accumulate_every=2, fp16=False, step_start_ema=2000, update_ema_every=10,
                  save_and_sample_every=5000, save_with_time_stamp_every=50000, results_folder='./results', load_path=None,
                  random_aug=False, torchvision_dataset=False, dataset=None, to_lab=False, order_seed=-1):
-        if to_lab:
-            raise NotImplementedError("to_lab (kornia Lab colour path) is out of scope of the H100 engine")
         core = _unwrap(diffusion_model)
         size = core.image_size
         self._size2 = tuple(size) if isinstance(size, (tuple, list)) else (size, size)
@@ -544,7 +551,12 @@ class SnowificationTrainer(SnowEvaluationMixin, Trainer):
                          save_and_sample_every=save_and_sample_every, results_folder=results_folder, load_path=load_path,
                          dataset=dataset, shuffle=True)
         self.results_folder.mkdir(parents=True, exist_ok=True)
-        self.post_process_func = lambda x: x
+        self.post_process_func = self._to_lab_on_device if to_lab else (lambda x: x)
+
+    @staticmethod
+    def _to_lab_on_device(x):
+        from .snowification import rgb2lab
+        return rgb2lab(x.cuda(non_blocking=True))
 
     def _make_loader(self, folder, dataset, shuffle, seed):
         if folder is None or dataset == 'synthetic':
@@ -564,7 +576,16 @@ class SnowificationTrainer(SnowEvaluationMixin, Trainer):
         return ds, gen()
 
     def _process_item(self, x):
-        return x[0] if isinstance(x, (list, tuple)) else x
+        return self.post_process_func(x[0] if isinstance(x, (list, tuple)) else x)
+
+    def _loss(self, d):
+        return super()._loss(self.post_process_func(d))
+
+    def _sample_start(self):
+        return self.post_process_func(super()._sample_start())
+
+    def _eval_batch(self):
+        return self.post_process_func(super()._eval_batch())
 
     def save(self, save_with_time_stamp=False):
         d = {'step': self.step, 'model': self.model.state_dict(), 'ema': self.ema_model.state_dict()}
@@ -585,6 +606,9 @@ class SnowificationTrainer(SnowEvaluationMixin, Trainer):
                 milestone = self.step // self.save_and_sample_every
                 og_img = self._sample_start()
                 sample_dict = _unwrap(self.ema_model).sample(batch_size=self.batch_size, img=og_img)
+                if self.to_lab:
+                    from .snowification import lab2rgb
+                    og_img = lab2rgb(og_img)
                 sample_dict['og'] = og_img
                 print(f'images saved: {sample_dict.keys()}')
                 for k, img in sample_dict.items():

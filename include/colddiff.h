@@ -323,6 +323,16 @@ int cd_chanmix(const float* xt, const float* xsrc, float* out, const float* mats
 int cd_snow(const float* xt, const float* og, float* out, const float* snow, const float* br_coef, const int64_t* t_hi,
             const int64_t* t_lo, int hi_off, int lo_off, int B, int H, int W, int snow_batch, int fix_brightness,
             int mode, void* stream);
+/* Lab colour path of the decolorization package (to_lab=True; diffusion/utils.py:113-222 "UT", FP:189-218).  NCHW, 3 channels.
+ * cd_lab_convert: to_lab = 1: rgb2lab (RGB in [-1, 1] -> L 0..100, a, b); to_lab = 0: lab2rgb(x, clip) -> 2 rgb - 1 (fz clamped
+ *   at 0, rgb clipped to [0, 1] when `clip`).  out == x is allowed.
+ * cd_chanmix_lab: the masked stepping of cd_chanmix (same t_hi / t_lo / offsets / modes) with D = the Lab step chain:
+ *   D(v, k) = step_k(... step_0(v)), step_i(v) = rgb2lab(step_mats[i] lab2rgb(v, clip=True)), step_mats = the PER-STEP [T][3][3]
+ *   table (not cumulative: the clamp and clip at every step make the chain nonlinear).  index < 0 = v untouched (no round trip).
+ * sRGB / XYZ stages restate kornia's formulas (unpinned upstream).                                                            */
+int cd_lab_convert(const float* x, float* out, int B, int64_t HW, int to_lab, int clip, void* stream);
+int cd_chanmix_lab(const float* xt, const float* xsrc, float* out, const float* step_mats, const int64_t* t_hi,
+                   const int64_t* t_lo, int hi_off, int lo_off, int B, int64_t HW, int mode, void* stream);
 /* Snow-layer generation (FP:32-42 clipped_zoom + FP:252-355 generate_snow_layer), everything after the host's random draws:
  *   base[s]  = fp32( trim( zoom_order1( noise[s] : ch x ch fp64 -> m x m ) ) )  : H x H, scipy.ndimage.zoom arithmetic, bit-exact
  *   snow[t][s][0..2] = motion_blur_t( clip( base[s] < thres[t] ? 0 : base[s], 0, 1 ) )
