@@ -57,7 +57,7 @@ if os.environ.get('COLDDIFF_2CTA') in ('0', '1', '2'):   # SM-pair (two-CTA clus
 lib.cd_last_error.argtypes = [C.c_char_p, C.c_size_t]
 if os.environ.get('COLDDIFF_CONV_TWO_CTAS') in ('0', '64', '128', '192'):   # two CTAs per SM for the N <= 128 convolution tiles (bit mask)
     lib.cd_conv_tc_set_two_ctas(int(os.environ['COLDDIFF_CONV_TWO_CTAS']))
-if os.environ.get('COLDDIFF_CONV_HALO') in ('0', '1', '2', '3', '6'):   # halo-tile kernel for the 3x3 convolutions (1: 16 x 8 tiles, 2: 16 x 16)
+if os.environ.get('COLDDIFF_CONV_HALO') in ('0', '1', '2', '6', '8'):   # 3x3 convolution kernel: 0 shape-based (default), 1 / 2 / 6 shared-row kernel, 8 per-tap kernel
     lib.cd_conv_tc_set_halo(int(os.environ['COLDDIFF_CONV_HALO']))
 if os.environ.get('COLDDIFF_2CTA_BN') in ('0', '64', '128', '192'):   # N tiles below 256 on the SM-pair kernel (bit mask 128 | 64)
     lib.cd_conv_tc_set_2cta_bn(int(os.environ['COLDDIFF_2CTA_BN']))

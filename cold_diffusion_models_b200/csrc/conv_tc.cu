@@ -43,6 +43,13 @@ struct TcParams {
   int act; int round_tf32;
   float* out2; int out2_ld;
   const float* aux; int aux_ld;
+  // shared-row kernel, per source: the dx of each box, the taps in column order (taps [boxend[b - 1], boxend[b]) read box b),
+  // and each of those taps' byte offset inside its box
+  int nbox[2];
+  int8_t boxdx[2][3];
+  int8_t boxend[2][3];
+  int8_t taporder[2][CD_MAX_TAPS];
+  int tapoff[2][CD_MAX_TAPS];
 };
 
 // output pixel of GEMM row m of tile `tile` (-1: beyond the batch)
@@ -241,63 +248,69 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
 }
 
 // ---------------------------------------------------------------------------------------------
-// Halo-tile kernel for stride-1 convolutions whose taps lie in [-1, 1]^2 (dense 3x3 forward / data gradient, fused [3x3 | 1x1]
-// pairs): a CTA tile is 16 x TH output pixels of one image (TH = 8: 128 GEMM rows, one 64-row accumulator per consumer
-// warpgroup; TH = 16: 256 rows, two accumulators per warpgroup that share every weight tile).  Per source and 32-channel chunk
-// ONE TMA box fetches the (16 + 2) x (TH + 2) halo patch; every tap reads its shifted window of that patch into registers as the
-// wgmma A operand (tf32, rounded to nearest), so activations leave L2 once per chunk instead of once per tap.  Weight tiles
-// stream through their own STAGES-deep ring.  Grids need not be powers of two: pixels outside the grid are masked.
+// Shared-row kernel for stride-1 convolutions whose taps lie in [-1, 1]^2 (dense 3x3 forward / data gradient, fused [3x3 | 1x1]
+// pairs).  A CTA tile is 16 x 8 = 128 output pixels of one image by 64 or 128 output channels.  Per source and 32-channel
+// chunk the producer fetches ONE 4-D TMA box {32 ch, 16, 8 + 2, 1} at (x0 + dx, y0 - 1) for each distinct tap column dx of
+// that source (three for a 3x3 source, one for a 1x1 source).  Box row r = (y + 1) * 16 + x holds pixel (x0 + dx + x, y0 + y),
+// so tap (dy, dx) reads the GEMM rows [64 w, 64 w + 64) of warpgroup w as the contiguous rows starting at (dy + 1) * 16 + 64 w
+// of the dx box: a wgmma descriptor offset by a multiple of 1024 bytes (one SW128 atom), no registers involved.  Activations leave L2 once per (chunk, dx) instead
+// of once per tap, and the TMA unit writes 160 pixel rows into shared memory per three taps instead of 3 x 128.
+// The taps run grouped by column (p.taporder), so a box is released as soon as the taps of its column have retired: boxes
+// stream through an ABOXES-deep ring, weight tiles through their own STAGES-deep ring.  Grids need not be multiples of the tile:
+// pixels outside the grid are zero-filled on load and masked in the epilogue.
 // ---------------------------------------------------------------------------------------------
-constexpr int kHaloW = 16;
+constexpr int kRowsTW = 16, kRowsTH = kTileM / kRowsTW;
+constexpr int kRowsBoxBytes = kRowsTW * (kRowsTH + 2) * 128;     // 20 KB: one tap column of one chunk
 
-template <int BN, int MB, int STAGES, int CTAS = 1>
+template <int BN, int ABOXES, int STAGES, int CTAS>
 __global__ void __launch_bounds__(kThreads, CTAS)
-conv_halo_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
-                 const __grid_constant__ CUtensorMap mapB0, const __grid_constant__ CUtensorMap mapB1, const TcParams p) {
-  constexpr int TH = 8 * MB;
-  constexpr int PW = kHaloW + 2, PH = TH + 2;
-  constexpr int kPatchBytes = (PW * PH * 128 + 1023) / 1024 * 1024;
+conv_rows_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
+                 const __grid_constant__ CUtensorMap mapB0, const __grid_constant__ CUtensorMap mapB1, const __grid_constant__ TcParams p) {
   constexpr int kBBytes = BN * 128;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  uint8_t* patch = smem;                                   // 2 patch slots
-  uint8_t* wtile = smem + 2 * kPatchBytes;                 // STAGES weight tiles
+  uint8_t* abox = smem;                                    // ABOXES activation boxes
+  uint8_t* wtile = smem + ABOXES * kRowsBoxBytes;          // STAGES weight tiles
   uint64_t* bars = reinterpret_cast<uint64_t*>(wtile + STAGES * kBBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* pfull = bars + 2 * STAGES;
-  uint64_t* pempty = bars + 2 * STAGES + 2;
+  uint64_t* afull = bars + 2 * STAGES;
+  uint64_t* aempty = bars + 2 * STAGES + ABOXES;
+  static_assert(2 * (STAGES + ABOXES) * 8 <= 256, "barrier block is 256 bytes");
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumerWarps); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&pfull[i], 1); mbar_init(&pempty[i], kConsumerWarps); }
+    for (int i = 0; i < ABOXES; ++i) { mbar_init(&afull[i], 1); mbar_init(&aempty[i], kConsumerWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
   if (warp == kConsumerWarps) {
+    // ===================== TMA producer: ONE elected thread =====================
     if (elect_one()) {
-      uint32_t stage = 0, ph = 0, pi = 0, pph = 0;
+      uint32_t stage = 0, ph = 0, ai = 0, aph = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int co_t = tile % p.tiles_co;
+        const int co0 = (tile % p.tiles_co) * BN;
         int mt = tile / p.tiles_co;
-        const int tx = mt % p.tiles_x; mt /= p.tiles_x;
-        const int ty = mt % p.tiles_y;
+        const int x0 = (mt % p.tiles_x) * kRowsTW; mt /= p.tiles_x;
+        const int y0 = (mt % p.tiles_y) * kRowsTH;
         const int n = mt / p.tiles_y;
         for (int s = 0; s < p.nsrc; ++s) {
           const CUtensorMap* mA = s ? &mapA1 : &mapA0;
           const CUtensorMap* mB = s ? &mapB1 : &mapB0;
           for (int kc = 0; kc < p.kchunks[s]; ++kc) {
-            mbar_wait(&pempty[pi], pph ^ 1u);
-            mbar_expect_tx(&pfull[pi], PW * PH * 128);
-            tma_load_4d(smem_u32(patch + pi * kPatchBytes), mA, &pfull[pi], kc * kChunkK, tx * kHaloW - 1, ty * TH - 1, n);
-            if (++pi == 2) { pi = 0; pph ^= 1u; }
-            for (int tap = 0; tap < p.ntaps[s]; ++tap) {
-              mbar_wait(&empty_bar[stage], ph ^ 1u);
-              mbar_expect_tx(&full_bar[stage], kBBytes);
-              tma_load_3d(smem_u32(wtile + stage * kBBytes), mB, &full_bar[stage], kc * kChunkK, co_t * BN, tap);
-              if (++stage == STAGES) { stage = 0; ph ^= 1u; }
+            for (int b = 0, i = 0; b < p.nbox[s]; ++b) {
+              mbar_wait(&aempty[ai], aph ^ 1u);
+              mbar_expect_tx(&afull[ai], kRowsBoxBytes);
+              tma_load_4d(smem_u32(abox + ai * kRowsBoxBytes), mA, &afull[ai], kc * kChunkK, x0 + p.boxdx[s][b], y0 - 1, n);
+              if (++ai == ABOXES) { ai = 0; aph ^= 1u; }
+              for (; i < p.boxend[s][b]; ++i) {
+                mbar_wait(&empty_bar[stage], ph ^ 1u);
+                mbar_expect_tx(&full_bar[stage], kBBytes);
+                tma_load_3d(smem_u32(wtile + stage * kBBytes), mB, &full_bar[stage], kc * kChunkK, co0, p.taporder[s][i]);
+                if (++stage == STAGES) { stage = 0; ph ^= 1u; }
+              }
             }
           }
         }
@@ -307,75 +320,58 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constan
     return;
   }
 
-  // consumers: warpgroup wg owns tile rows [64 MB wg, 64 MB (wg + 1)); row m = pixel (m % 16, m / 16) of the tile
+  // ===================== consumers: warpgroup wg owns GEMM rows [64 wg, 64 wg + 64); row m = pixel (m % 16, m / 16) =====================
   const int tid = threadIdx.x & 127;
   const int rl = (tid >> 5) * 16 + (lane >> 2);
-  const int q2 = (lane & 3) * 2, t4 = lane & 3;
-  int prow[MB][2];                                   // patch row of this lane's two A rows per block, tap (0, 0) of the window
-#pragma unroll
-  for (int mb = 0; mb < MB; ++mb)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m = (wg * MB + mb) * 64 + rl + 8 * h;
-      prow[mb][h] = (m / kHaloW + 1) * PW + (m % kHaloW) + 1;
-    }
-  float acc[MB][BN / 2];
-  uint32_t stage = 0, ph = 0, pi = 0, pph = 0;
+  const int q2 = (lane & 3) * 2;
+  auto release = [&](uint64_t* bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
+  float acc[BN / 2];
+  uint32_t stage = 0, ph = 0, ai = 0, aph = 0;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-    bool first = true;
+    int k = 0;
+    uint32_t prev = 0, prev_a = 0;
     for (int s = 0; s < p.nsrc; ++s) {
       for (int kc = 0; kc < p.kchunks[s]; ++kc) {
-        mbar_wait(&pfull[pi], pph);
-        const uint8_t* pt = patch + pi * kPatchBytes;
-        for (int tap = 0; tap < p.ntaps[s]; ++tap) {
-          const int shift = p.dy[s][tap] * PW + p.dx[s][tap];
-          uint32_t a[MB][4][4];
-#pragma unroll
-          for (int mb = 0; mb < MB; ++mb)
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int row = prow[mb][e & 1] + shift, c = kk * 8 + t4 + 4 * (e >> 1);
-                a[mb][kk][e] = __float_as_uint(cd_round_tf32(
-                    *reinterpret_cast<const float*>(pt + row * 128 + ((((c >> 2) ^ row) & 7) << 4) + (c & 3) * 4)));
-              }
-          mbar_wait(&full_bar[stage], ph);
-          wgmma_fence();
-          const uint64_t db = make_kmajor_sw128_desc(smem_u32(wtile + stage * kBBytes));
-#pragma unroll
-          for (int mb = 0; mb < MB; ++mb)
+        for (int b = 0, i = 0; b < p.nbox[s]; ++b) {
+          mbar_wait(&afull[ai], aph);
+          const uint32_t abase = smem_u32(abox + ai * kRowsBoxBytes) + wg * (kABytes / 2);
+          for (const int i0 = i; i < p.boxend[s][b]; ++i, ++k) {
+            mbar_wait(&full_bar[stage], ph);
+            wgmma_fence();
+            const uint64_t da = make_kmajor_sw128_desc(abase + p.tapoff[s][i]);
+            const uint64_t db = make_kmajor_sw128_desc(smem_u32(wtile + stage * kBBytes));
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk)
-              wgmma_tf32_rs<BN>(acc[mb], a[mb][kk], db + uint64_t(kk * 2), (first && kk == 0) ? 0u : 1u);
-          wgmma_commit();
-          wgmma_wait<0>();                         // the A registers are reloaded for the next tap
-          first = false;
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; ph ^= 1u; }
+              wgmma_tf32<BN>(acc, da + uint64_t(kk * 2), db + uint64_t(kk * 2), (k | kk) != 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<1>();                         // the previous tap's MMAs have retired
+            if (k > 0) release(&empty_bar[prev]);
+            if (k > 0 && i == i0) release(&aempty[prev_a]);   // ... and with them every tap of the previous box
+            prev = stage;
+            if (++stage == STAGES) { stage = 0; ph ^= 1u; }
+          }
+          prev_a = ai;
+          if (++ai == ABOXES) { ai = 0; aph ^= 1u; }
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&pempty[pi]);
-        if (++pi == 2) { pi = 0; pph ^= 1u; }
       }
     }
-    const int co_t = tile % p.tiles_co, co0 = co_t * BN;
+    wgmma_wait<0>();
+    if (k > 0) { release(&empty_bar[prev]); release(&aempty[prev_a]); }
+
+    const int co0 = (tile % p.tiles_co) * BN;
     int mt = tile / p.tiles_co;
-    const int tx = mt % p.tiles_x; mt /= p.tiles_x;
-    const int ty = mt % p.tiles_y;
+    const int x0 = (mt % p.tiles_x) * kRowsTW; mt /= p.tiles_x;
+    const int y0 = (mt % p.tiles_y) * kRowsTH;
     const int n = mt / p.tiles_y;
 #pragma unroll
-    for (int mb = 0; mb < MB; ++mb)
+    for (int h = 0; h < 2; ++h) {
+      const int m = wg * 64 + rl + 8 * h;
+      const int gx = x0 + m % kRowsTW, gy = y0 + m / kRowsTW;
+      if (gx >= p.Wg || gy >= p.Hg) continue;
+      const long long pix = (static_cast<long long>(n) * p.Ho + (gy * p.oys + p.oy0)) * p.Wo + (gx * p.oxs + p.ox0);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int m = (wg * MB + mb) * 64 + rl + 8 * h;
-        const int gx = tx * kHaloW + m % kHaloW, gy = ty * TH + m / kHaloW;
-        if (gx >= p.Wg || gy >= p.Hg) continue;
-        const long long pix = (static_cast<long long>(n) * p.Ho + (gy * p.oys + p.oy0)) * p.Wo + (gx * p.oxs + p.ox0);
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) epi_pair(p, pix, co0 + 8 * j + q2, acc[mb][4 * j + 2 * h], acc[mb][4 * j + 2 * h + 1]);
-      }
+      for (int j = 0; j < BN / 8; ++j) epi_pair(p, pix, co0 + 8 * j + q2, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    }
   }
 }
 
@@ -416,20 +412,20 @@ int launch(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
   return 0;
 }
 
-template <int BN, int MB, int STAGES, int CTAS = 1>
-int launch_halo(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
-  constexpr int kPatchBytes = ((kHaloW + 2) * (8 * MB + 2) * 128 + 1023) / 1024 * 1024;
-  constexpr size_t smem = 2 * size_t(kPatchBytes) + size_t(STAGES) * BN * 128 + 1024 + 256;
+template <int BN, int ABOXES, int STAGES, int CTAS = 1>
+int launch_rows(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
+  constexpr size_t smem = size_t(ABOXES) * kRowsBoxBytes + size_t(STAGES) * BN * 128 + 1024 + 256;
   static_assert(smem <= 232448, "dynamic shared memory of one CTA (227 KB)");
   static_assert(CTAS == 1 || 2 * (smem + 1024) <= 233472, "two CTAs per SM must fit the 228 KB of shared memory");
+  auto kern = conv_rows_kernel<BN, ABOXES, STAGES, CTAS>;
   static bool attr_done = false;
   if (!attr_done) {
-    CD_CUDA(cudaFuncSetAttribute(conv_halo_kernel<BN, MB, STAGES, CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CD_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_done = true;
   }
   const int slots = g_num_sms * CTAS;
   const int grid = p.total_tiles < slots ? p.total_tiles : slots;
-  conv_halo_kernel<BN, MB, STAGES, CTAS><<<grid, kThreads, smem, st>>>(maps[0], maps[1], maps[2], maps[3], p);
+  kern<<<grid, kThreads, smem, st>>>(maps[0], maps[1], maps[2], maps[3], p);
   CD_LAUNCH_CHECK();
   return 0;
 }
@@ -438,18 +434,20 @@ int launch_halo(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
 
 extern "C" int cd_conv_tc_set_tf32_maps(int enable) { g_tf32_map_dtype = enable ? 1 : 0; return 0; }
 
-// Defaults measured with tools/conv_shapes.py and bench.py on an H100 80GB HBM3 at a 400 W power limit (Unet config 3, batch 32):
-// convolution forward time per training step 80 ms with the per-tap kernel at one CTA per SM, 74 ms with two CTAs per SM for the
-// 64- and 128-wide N tiles (375 -> 387 images/s), 87 ms with the SM-pair kernel, 86 / 95 ms with the 16 x 8 / 16 x 16 halo-tile
-// kernel.  So two CTAs per SM is on by default; the pair and halo variants are off.
+// Defaults measured with tools/conv_shapes.py and bench.py on an H100 80GB HBM3 at a 400 W power limit (Unet config 3, batch 32).
+// Per-tap kernel: 80 ms of convolution forward + data-gradient time per training step at one CTA per SM, 74 ms with two CTAs per
+// SM for the 64- and 128-wide N tiles (375 -> 387 images/s); the SM-pair kernel took 87 ms.  The shared-row kernel cuts the
+// modelled L2 -> SM bytes of the 3x3 layers 1.2-1.6x; what gains most, though, is that its 128-wide N tiles fit two CTAs per SM
+// for the layers with Cout >= 256 too (a CTA's epilogue then overlaps the other's mainloop): 20-48 % faster on those layers
+// than the per-tap kernel's 256-wide tiles, 0-10 % on the narrower ones.  16 x 16 pixel tiles (two accumulators per weight tile, one CTA per SM) were slower on every layer.
+// A single wave of tiles (16^2, Cout = 256) stays per-tap, and two CTAs per SM are used only with more than one wave of tiles.
 static int g_use_2cta = 0;
 extern "C" int cd_conv_tc_set_2cta(int mode) { g_use_2cta = mode; return 0; }   // 0 off, 1 where the cost model prefers it, 2 wherever eligible
 // narrower pair tiles: bit mask of the N tiles below 256 (128 | 64) that go to the SM-pair kernel when the problem is eligible
 static int g_2cta_bn = 0;
 extern "C" int cd_conv_tc_set_2cta_bn(int mask) { g_2cta_bn = mask & (128 | 64); return 0; }
-// halo-tile kernel for stride-1 convolutions with taps in [-1, 1]^2, bit mask: 1 = 16 x 8 pixel tiles wherever eligible,
-// 2 = 16 x 16 tiles (two accumulators per weight tile) for Cout <= 128 on grids of at least 32 x 32, 4 (with 2) = 16 x 16 tiles
-// for every eligible problem (tests); 0 = off (default)
+// kernel for stride-1 convolutions with taps in [-1, 1]^2: 0 = shape-based choice between the shared-row and the per-tap kernel
+// (default), 1, 2 or 6 = shared-row kernel wherever eligible, 8 = per-tap kernel everywhere
 static int g_use_halo = 0;
 extern "C" int cd_conv_tc_set_halo(int enable) { g_use_halo = enable; return 0; }
 // two CTAs per SM (half the stages each) for N <= 128: bit mask of N tiles (128 | 64)
@@ -485,16 +483,15 @@ extern "C" int cd_conv_fwd_f16_probe(const CdConvDesc* d, void* stream) {
   return conv_fwd_tc_impl(d, static_cast<cudaStream_t>(stream), true);
 }
 
-static int conv_fwd_halo(const CdConvDesc* d, cudaStream_t st, int MB);
+static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, bool by_shape);
 
 static int conv_fwd_tc_impl(const CdConvDesc* d, cudaStream_t st, bool f16) {
-  if (!f16 && g_epi_staged == 0 && (g_use_halo & 2)) {
-    const int r = conv_fwd_halo(d, st, 2);
-    if (r <= 0) return r;                                     // 1 = not eligible
-  }
-  if (!f16 && g_epi_staged == 0 && (g_use_halo & 1)) {
-    const int r = conv_fwd_halo(d, st, 1);
-    if (r <= 0) return r;
+  if (!f16 && g_epi_staged == 0) {
+    // shared-row kernel: chosen by shape (0; the SM-pair switch keeps the per-tap family) or wherever eligible (1, 2, 6)
+    if ((g_use_halo == 0 && !g_use_2cta) || g_use_halo == 1 || g_use_halo == 2 || g_use_halo == 6) {
+      const int r = conv_fwd_rows(d, st, g_use_halo == 0);
+      if (r <= 0) return r;                                   // 1 = not eligible
+    }
   }
   const int chunk_elems = f16 ? 64 : kChunkK;
   const int esz = f16 ? 2 : 4;
@@ -599,14 +596,18 @@ static int conv_fwd_tc_impl(const CdConvDesc* d, cudaStream_t st, bool f16) {
     if (BN == 128) return launch<128, 6, false, false, 1, true>(maps, p, st);
     return launch<64, 8, false, false, 1, true>(maps, p, st);
   }
+  // two CTAs per SM only with more than one wave of tiles: a single wave would pair CTAs on some SMs and leave others idle
+  const int ctas2 = p.total_tiles > g_num_sms ? g_ctas2 : 0;
   if (BN == 256) return launch<256, 4>(maps, p, st);
-  if (BN == 128) return (g_ctas2 & 128) ? launch<128, 3, false, false, 2>(maps, p, st) : launch<128, 6>(maps, p, st);
-  return (g_ctas2 & 64) ? launch<64, 4, false, false, 2>(maps, p, st) : launch<64, 8>(maps, p, st);
+  if (BN == 128) return (ctas2 & 128) ? launch<128, 3, false, false, 2>(maps, p, st) : launch<128, 6>(maps, p, st);
+  return (ctas2 & 64) ? launch<64, 4, false, false, 2>(maps, p, st) : launch<64, 8>(maps, p, st);
 }
 
-// returns 1 when the problem is not eligible for the halo-tile kernel (MB = 1: 16 x 8 tiles, 2: 16 x 16 tiles)
-static int conv_fwd_halo(const CdConvDesc* d, cudaStream_t st, int MB) {
-  if (d->sy != 1 || d->sx != 1 || d->nsrc < 1 || d->nsrc > 2 || !g_tf32_map_dtype) return 1;
+// returns 1 when the problem is not eligible for the shared-row kernel -- it needs stride 1, taps in [-1, 1]^2 and a first source
+// whose tap columns hold three taps each on average (dense 3x3; 1x1 and transposed-convolution parity tap lists stay per-tap) --
+// or, with by_shape, when the per-tap kernel is the faster one for this shape (see the measurement above g_use_2cta)
+static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, bool by_shape) {
+  if (d->sy != 1 || d->sx != 1 || d->nsrc < 1 || d->nsrc > 2) return 1;
   for (int s = 0; s < d->nsrc; ++s) {
     const CdConvSrc& cs = d->s[s];
     if (cs.w_per_batch || cs.C % kChunkK != 0 || cs.C <= 0 || cs.ntaps < 1 || cs.ntaps > CD_MAX_TAPS) return 1;
@@ -614,7 +615,6 @@ static int conv_fwd_halo(const CdConvDesc* d, cudaStream_t st, int MB) {
     for (int t = 0; t < cs.ntaps; ++t) if (cs.dy[t] < -1 || cs.dy[t] > 1 || cs.dx[t] < -1 || cs.dx[t] > 1) return 1;
     if ((reinterpret_cast<uintptr_t>(cs.src) & 15) || (cs.ld * 4) % 16 || (reinterpret_cast<uintptr_t>(cs.w) & 15)) return 1;
   }
-  if (MB == 2 && (d->Cout > 128 || (!(g_use_halo & 4) && (d->Hg < 32 || d->Wg < 32)))) return 1;
   if ((reinterpret_cast<uintptr_t>(d->out) & 15) || d->out_ld % 4) return 1;
   if (d->resid && ((reinterpret_cast<uintptr_t>(d->resid) & 15) || d->resid_ld % 4)) return 1;
   if (d->out2 && ((reinterpret_cast<uintptr_t>(d->out2) & 15) || d->out2_ld % 4)) return 1;
@@ -626,46 +626,61 @@ static int conv_fwd_halo(const CdConvDesc* d, cudaStream_t st, int MB) {
     int dev = 0; CD_CUDA(cudaGetDevice(&dev));
     CD_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
   }
-  const int BN = (d->Cout % 256 == 0 && MB == 1) ? 256 : (d->Cout > 64 ? 128 : 64);
-  const int TH = 8 * MB;
   TcParams p{};
   p.B = d->B; p.Hg = d->Hg; p.Wg = d->Wg; p.sy = 1; p.sx = 1; p.Cout = d->Cout; p.nsrc = d->nsrc;
-  p.TW = kHaloW; p.TH = TH; p.TN = 1;
-  p.tiles_x = cd_cdiv(d->Wg, kHaloW); p.tiles_y = cd_cdiv(d->Hg, TH); p.tiles_n = d->B;
+  p.TW = kRowsTW; p.TH = kRowsTH; p.TN = 1;
+  p.tiles_x = cd_cdiv(d->Wg, kRowsTW); p.tiles_y = cd_cdiv(d->Hg, kRowsTH); p.tiles_n = d->B;
+  // N tiles of at most 128 columns: two CTAs per SM fit (three boxes and three / six weight tiles each), so one CTA's epilogue
+  // overlaps the other's mainloop.  For the layers with Cout >= 256 this beats the 256-wide tile at one CTA per SM by 20-45 %,
+  // although every activation box is then fetched once per 128 output channels.
+  const int BN = d->Cout > 64 ? 128 : 64;
   p.tiles_co = cd_cdiv(d->Cout, BN);
   p.total_tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.tiles_co;
+  // by shape: when the tiles fill more than one wave (a single wave, e.g. the 16^2 layers with Cout = 256, runs faster on the
+  // per-tap kernel)
+  if (by_shape && p.total_tiles <= g_num_sms) return 1;
   p.out = d->out; p.out_ld = d->out_ld; p.Ho = d->Ho; p.Wo = d->Wo;
   p.oys = d->oys; p.oxs = d->oxs; p.oy0 = d->oy0; p.ox0 = d->ox0;
   p.bias = d->bias; p.resid = d->resid; p.resid_ld = d->resid_ld; p.act = d->act; p.round_tf32 = d->round_tf32;
   p.out2 = d->out2; p.out2_ld = d->out2_ld; p.aux = d->aux; p.aux_ld = d->aux_ld;
+  const CUtensorMapDataType dt = g_tf32_map_dtype ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUtensorMap maps[4];
   for (int s = 0; s < 2; ++s) {
     const CdConvSrc& cs = d->s[s < d->nsrc ? s : 0];
     p.ntaps[s] = cs.ntaps; p.kchunks[s] = cs.C / kChunkK; p.wpb[s] = 0;
+    p.nbox[s] = 0;
+    int i = 0;
+    for (int dx = -1; dx <= 1; ++dx) {                       // taps grouped by column: one box per column present
+      const int i0 = i;
+      for (int t = 0; t < cs.ntaps; ++t)
+        if (cs.dx[t] == dx) { p.taporder[s][i] = (int8_t)t; p.tapoff[s][i] = (cs.dy[t] + 1) * kRowsTW * 128; ++i; }
+      if (i > i0) { p.boxdx[s][p.nbox[s]] = (int8_t)dx; p.boxend[s][p.nbox[s]] = (int8_t)i; ++p.nbox[s]; }
+    }
+    if (s == 0 && cs.ntaps < 3 * p.nbox[0]) return 1;
     for (int t = 0; t < cs.ntaps; ++t) { p.dy[s][t] = (int8_t)cs.dy[t]; p.dx[s][t] = (int8_t)cs.dx[t]; }
-    {   // A: NHWC activations, one halo patch {32 ch, 18, TH + 2, 1} per chunk
+    {   // A: NHWC activations, one box {32 ch, 16, 8 + 2, 1} per chunk and tap column
       cuuint64_t dims[4] = {(cuuint64_t)cs.C, (cuuint64_t)cs.W, (cuuint64_t)cs.H, (cuuint64_t)d->B};
       cuuint64_t strides[3] = {(cuuint64_t)cs.ld * 4, (cuuint64_t)cs.ld * 4 * cs.W, (cuuint64_t)cs.ld * 4 * cs.W * cs.H};
-      cuuint32_t box[4] = {(cuuint32_t)kChunkK, (cuuint32_t)(kHaloW + 2), (cuuint32_t)(TH + 2), 1};
+      cuuint32_t box[4] = {(cuuint32_t)kChunkK, (cuuint32_t)kRowsTW, (cuuint32_t)(kRowsTH + 2), 1};
       cuuint32_t estr[4] = {1, 1, 1, 1};
-      CUresult r = enc(&maps[s], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(cs.src), dims, strides, box, estr,
+      CUresult r = enc(&maps[s], dt, 4, const_cast<float*>(cs.src), dims, strides, box, estr,
                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(halo A%d) failed: %d", s, (int)r);
+      CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(rows A%d) failed: %d", s, (int)r);
     }
     {   // B: packed weights [tap][Cout][Cin]
       cuuint64_t dims[3] = {(cuuint64_t)cs.C, (cuuint64_t)d->Cout, (cuuint64_t)cs.ntaps};
       cuuint64_t strides[2] = {(cuuint64_t)cs.C * 4, (cuuint64_t)cs.C * 4 * d->Cout};
       cuuint32_t box[3] = {(cuuint32_t)kChunkK, (cuuint32_t)BN, 1};
       cuuint32_t estr[3] = {1, 1, 1};
-      CUresult r = enc(&maps[2 + s], CU_TENSOR_MAP_DATA_TYPE_TFLOAT32, 3, const_cast<float*>(cs.w), dims, strides, box, estr,
+      CUresult r = enc(&maps[2 + s], dt, 3, const_cast<float*>(cs.w), dims, strides, box, estr,
                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(halo B%d) failed: %d", s, (int)r);
+      CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(rows B%d) failed: %d", s, (int)r);
     }
   }
-  if (MB == 2) return BN == 128 ? launch_halo<128, 2, 4>(maps, p, st) : launch_halo<64, 2, 6>(maps, p, st);
-  if (BN == 256) return launch_halo<256, 1, 4>(maps, p, st);
-  if (BN == 128) return (g_ctas2 & 128) ? launch_halo<128, 1, 2, 2>(maps, p, st) : launch_halo<128, 1, 6>(maps, p, st);
-  return (g_ctas2 & 64) ? launch_halo<64, 1, 3, 2>(maps, p, st) : launch_halo<64, 1, 8>(maps, p, st);
+  // one CTA per SM: six boxes (120 KB) and 64 KB of weight tiles; two CTAs per SM: three boxes and 48 KB of weight tiles each
+  const int ctas2 = p.total_tiles > g_num_sms ? g_ctas2 : 0;
+  if (BN == 128) return (ctas2 & 128) ? launch_rows<128, 3, 3, 2>(maps, p, st) : launch_rows<128, 6, 4>(maps, p, st);
+  return (ctas2 & 64) ? launch_rows<64, 3, 6, 2>(maps, p, st) : launch_rows<64, 6, 8>(maps, p, st);
 }
