@@ -59,6 +59,8 @@ if os.environ.get('COLDDIFF_CONV_TWO_CTAS') in ('0', '64', '128', '192'):   # tw
     lib.cd_conv_tc_set_two_ctas(int(os.environ['COLDDIFF_CONV_TWO_CTAS']))
 if os.environ.get('COLDDIFF_CONV_HALO') in ('0', '1', '2', '6', '8'):   # 3x3 convolution kernel: 0 shape-based (default), 1 / 2 / 6 shared-row kernel, 8 per-tap kernel
     lib.cd_conv_tc_set_halo(int(os.environ['COLDDIFF_CONV_HALO']))
+if os.environ.get('COLDDIFF_WGRAD_MODE') in ('0', '1', '8'):   # tensor-core weight gradient: 1 wgmma kernel where eligible (default), 8 mma.sync halo kernel, 0 mma.sync one X tile per tap
+    lib.cd_wgrad_tc_set_mode(int(os.environ['COLDDIFF_WGRAD_MODE']))
 if os.environ.get('COLDDIFF_2CTA_BN') in ('0', '64', '128', '192'):   # N tiles below 256 on the SM-pair kernel (bit mask 128 | 64)
     lib.cd_conv_tc_set_2cta_bn(int(os.environ['COLDDIFF_2CTA_BN']))
 if os.environ.get('COLDDIFF_CONV_STAGED_EPILOGUE') in ('0', '1', '2', '3'):   # line-coalesced conv epilogue (csrc/conv_epilogue.cuh); default 0

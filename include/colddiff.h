@@ -189,7 +189,9 @@ int cd_conv1x1_to_nchw(const float* x, int ld, int B, int H, int W, int C, const
 int cd_nchw_to_nhwc(const float* x, int B, int C, int H, int W, float* out, int ld, void* stream);
 /* out[c] += sum_rows x[row*ld + c]  (bias / LayerNorm-beta gradients) */
 int cd_colsum(const float* x, int ld, int64_t rows, int C, float* out, void* stream);
-/* diagnostic switch for the tensor-core wgrad: 0 = one X tile per tap, otherwise (default) the dx taps of a 3x3 kernel share one halo tile */
+/* kernel switch of the tensor-core wgrad: 0 = mma.sync kernel with one X tile per tap; 8 = mma.sync kernel whose dx taps of a 3x3
+ * kernel share one halo tile; any other value (default 1) = the wgmma kernel for stride-1 problems with taps in [-1, 1]^2, one weight
+ * set, Cin % 64 == 0 and Cout % 64 == 0 (and no bias fusion), the mma.sync halo kernel for the rest */
 int cd_wgrad_tc_set_mode(int mode);
 /* K-split policy of the tensor-core wgrad: 0 = two waves rounded up, 1 / 2 = at most one / two full waves of CTAs,
  * 3 (default) = minimise waves x (chunks_per_split x t_chunk + over_clk); over_clk > 0 sets the per-CTA fixed cost (SM clocks) */
