@@ -5,9 +5,10 @@
 //
 // as a GEMM whose K dimension is the PIXEL axis.  NHWC rows hold the channels contiguously, i.e. both operands are
 // MN-major, which TF32 wgmma cannot read from shared memory.  Two kernels:
-//  - wgrad_wgmma_kernel (stride-1 taps in [-1, 1]^2, one weight set, Cin and Cout multiples of 64: the dense 3x3 layers) feeds
-//    wgmma with X from registers and with dY transposed once per pixel chunk into a K-major tile (see its comment below);
-//  - wgrad_tc_kernel, for everything else (strided, transposed-convolution parity, per-batch, image edge, bias fusion), below.
+//  - wgrad_wgmma_kernel (every weight gradient of the Unet: 3x3, 1x1, the per-batch attention product, the 4x4 stride-2
+//    downsample by input-parity class, the transposed-convolution parity problems and the Cin = 32 image edge) feeds wgmma with X
+//    from registers and with dY transposed once per pixel chunk into a K-major tile (see its comment below);
+//  - wgrad_tc_kernel, for the opt-in bias fusion, the forced modes 0 / 8 and problems the wgmma kernel does not take, below.
 // wgrad_tc_kernel runs mma.sync.m16n8k8 (TF32, fp32 accumulate) with its fragments read from the swizzled TMA tiles.
 // dY tiles ({32 co, CW px, R rows} TMA boxes) and
 // X tiles land in SWIZZLE_128B shared memory.  One CTA owns (co tile, ci tile, tap group, pixel split) and keeps one
@@ -44,6 +45,11 @@ struct WgParams {
   long long dw_batch_stride;
   float* dw;
   float* db;                      // BIAS kernels only: db[co] += sum over all pixels of dY (nullptr: not fused)
+  // wgmma kernel: a CTA covers ci_tile input channels from ci0; group g loads wm_nbox[g] X boxes of 32 channels (ci0 + 32 j) per chunk; accumulator slot t of the
+  // group is an m64 tile whose half h (warps 2h, 2h + 1: 32 rows) reads box wm_box[g][t][h] at pixel-row offset wm_shift[g][t][h]
+  // and belongs to tap wm_tap[g][t][h] (-1: idle half)
+  int wm_nbox[kMaxGroups], ci_tile;
+  int wm_box[kMaxGroups][kMaxTaps][2], wm_shift[kMaxGroups][kMaxTaps][2], wm_tap[kMaxGroups][kMaxTaps][2];
 };
 
 // element (row, c) of a 32-channel SWIZZLE_128B tile whose base is 1024-byte aligned: 16-byte chunk index XOR row % 8
@@ -215,7 +221,8 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_constant
 }
 
 // ---------------------------------------------------------------------------------------------
-// wgmma kernel for stride-1 convolutions whose taps lie in [-1, 1]^2 (dense 3x3), one weight set, Cin % 64 == 0, Cout % 64 == 0:
+// wgmma kernel for stride-1 problems whose taps lie in [-1, 1]^2, Cin % 64 == 0 or Cin == 32, Cout % 64 == 0 (see wgrad_wgmma for
+// how strided and parity problems are mapped onto it):
 //
 //   dW[tap][co][ci] += sum_q X[q + tap][ci] * dY[q][co]     M = 64 ci (A = X, registers), N = BN co (B = dY^T, shared memory)
 //
@@ -225,16 +232,19 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_constant
 //    boxes {32 co, CW, R, 1} (pixel-major, SWIZZLE_128B);
 //  - the transposer warpgroup rewrites dY as a K-major SWIZZLE_128B tile (rows = co, 128 bytes = 32 pixels), rounded RN to TF32,
 //    and hands it to the consumers through the async proxy;
-//  - consumer warpgroup w runs taps [w NT, w NT + NT) of the CTA's tap group: tap (dy, dx) reads its A fragment from the X box at
-//    a row offset (a register load is a free transpose), rounds it RN to TF32 and issues wgmma m64nBNk8 against the shared
-//    transposed dY tile.  A-fragment registers are double-buffered across k-steps (wgmma_wait<1>).
+//  - the consumer warpgroups split the accumulator slots of the CTA's group (ceil(n / 2) and the rest): a slot reads its A
+//    fragment from an X box at a row offset (a register load is a free transpose), rounds it RN to TF32 and issues wgmma m64nBNk8
+//    against the shared transposed dY tile.  A-fragment registers are double-buffered across k-steps (wgmma_wait<1>).
+//    A slot is one tap of 64 ci (3x3, halves from the two 32-ci boxes), one 64-ci block of a 1x1 (up to wm_slots_1x1 blocks per
+//    CTA, no halo: box {32 ci, CW, R}) or, at Cin = 32, two taps (one per 32-row half; the last half of an odd tap count idles).
 // Inside each k8 step the eight pixels are ordered 0 2 4 6 1 3 5 7 in A and B alike: the four lanes of a quad then read pixel
 // rows of four different swizzle phases, and the A loads are free of bank conflicts.
 // Partial sums of the pixel splits are combined with red.global.add into the packed [tap][Cout][Cin] gradient.
 // Warp roles (512 threads): warpgroup 0 = TMA producer (warp 0), warpgroup 1 = transposer, warpgroups 2-3 = consumers;
-// setmaxnreg moves the registers of the first two to the consumers (ptxas: 188 registers in a consumer of two m64n128 taps, 214 with four m64n64 taps; no spills).
+// setmaxnreg moves the registers of the first two to the consumers (ptxas, sm_90a: no spills and no serialized wgmma in any
+// instantiation).
 // CTA tile 64 ci x 128 co with two taps per consumer warpgroup (taps on grid z as {4, 4, 1}); Cout = 64: 64 ci x 64 co with four
-// taps per warpgroup ({8, 1}).  Measured with tools/wgrad_shapes.py on an H100 80GB HBM3 at a 700 W power limit (1980 MHz, Unet
+// taps per warpgroup ({8, 1}).  3x3 shapes measured with tools/wgrad_shapes.py on an H100 80GB HBM3 at a 700 W power limit (1980 MHz, Unet
 // config 3, batch 32): 160-220 TFLOP/s on the 3x3 shapes (133 at Cout = 64) against 46-91 for the mma.sync halo kernel; the 3x3
 // weight gradients of one backward take 10.0 ms instead of 24.6 ms.
 // ---------------------------------------------------------------------------------------------
@@ -242,10 +252,10 @@ constexpr int kWmThreads = 512;
 constexpr int kWmKR = 64;                      // pixels per chunk
 constexpr int kWmRegsLow = 40, kWmRegsHigh = 216;   // 128 x (40 + 40) + 256 x 216 <= 64 K registers
 
-template <int CW> struct WmGeom {
-  static constexpr int R = kWmKR / CW, RL = CW + 8;
-  static constexpr int kXBox = RL * (R + 2) * 128;         // one 32-ci X box
-  static constexpr int kXBytes = 2 * kXBox;                // 64 ci
+// HALO: the X box carries the halo of taps in [-1, 1]^2 ({32, CW + 8, R + 2}); otherwise (one tap at (0, 0)) it is the chunk itself
+template <int CW, bool HALO> struct WmGeom {
+  static constexpr int R = kWmKR / CW, RL = HALO ? CW + 8 : CW;
+  static constexpr int kXBox = RL * (R + (HALO ? 2 : 0)) * 128;   // one 32-ci X box
   static_assert(kXBox % 1024 == 0, "X boxes keep 1024-byte alignment");
 };
 template <int BN> struct WmTiles {
@@ -253,26 +263,36 @@ template <int BN> struct WmTiles {
   static constexpr int kRawBytes = (BN / 32) * kRawBox;
   static constexpr int kBBytes = BN * kWmKR * 4;           // transposed dY: kWmKR / 32 atoms of BN rows x 128 bytes
 };
+// 1x1: up to this many 64-ci slots per CTA share one transposed dY tile (as many as keep two stages in shared memory)
+constexpr int wm_slots_1x1(int BN) { return BN == 128 ? 3 : 4; }
+// one pipeline stage: [raw dY boxes | transposed dY | X boxes]; a 3x3 CTA loads two halo boxes (64 ci; one at Cin = 32), a 1x1
+// CTA up to 2 wm_slots_1x1 chunk boxes
+template <int BN, int CW, bool HALO> struct WmStage {
+  static constexpr int kXBytes = (HALO ? 2 : 2 * wm_slots_1x1(BN)) * WmGeom<CW, HALO>::kXBox;
+  static constexpr int kBytes = WmTiles<BN>::kRawBytes + WmTiles<BN>::kBBytes + kXBytes;
+  static_assert((224 * 1024) / kBytes >= 2, "two stages of the wgmma weight-gradient kernel fit shared memory");
+};
 
-template <int BN, int NTW, int CW>
-__device__ __forceinline__ void wm_consume(const WgParams& p, const uint8_t* smem, int stages, int stage_bytes, uint64_t* afull,
-                                           uint64_t* aempty, uint64_t* bfull, uint64_t* bempty, int nchunks, int g, int tbeg,
-                                           int co0, int ci0) {
-  using G = WmGeom<CW>;
+template <int BN, int NTW, int CW, bool HALO>
+__device__ __forceinline__ void wm_consume(const WgParams& p, const uint8_t* smem, int stages, int stage_bytes,
+                                           uint64_t* afull, uint64_t* aempty, uint64_t* bfull, uint64_t* bempty, int nchunks, int g,
+                                           int tbeg, int co0, int ci0) {
+  using G = WmGeom<CW, HALO>;
   using T = WmTiles<BN>;
   const int lane = threadIdx.x & 31, w = (threadIdx.x & 127) >> 5, gq = lane >> 2, tq = lane & 3;
-  // byte offsets inside a stage's X tile of this thread's A elements: a[0] / a[1] = pixel 2 tq, ci c / c + 8; a[2] / a[3] =
-  // pixel 2 tq + 1 (the k-step's first pixel row in the box at row offset tap_shift)
-  int off[NTW][4];
+  // byte offsets inside a stage's X boxes of this thread's A elements: a[0] / a[1] = pixel 2 tq, ci c / c + 8; a[2] / a[3] =
+  // pixel 2 tq + 1 (the k-step's first pixel row in box wm_box at row offset wm_shift)
+  int off[NTW][2];
   const int c = 16 * (w & 1) + gq;
 #pragma unroll
   for (int t = 0; t < NTW; ++t) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int row = p.tap_shift[g][tbeg + t] + 2 * tq + h;
-      const int o = (w >> 1) * G::kXBox + row * 128 + ((((c >> 2) ^ row) & 7) << 4) + (c & 3) * 4;
-      off[t][2 * h] = o;
-      off[t][2 * h + 1] = o ^ 32;                          // ci + 8: 16-byte chunk index + 2 (c >> 2 has bit 1 clear)
+      // the box of half w >> 1 follows from the slot layout (see wm_plan): 3x3 boxes 0 / 1, 1x1 boxes 2 t / 2 t + 1, Cin = 32 box 0
+      // with a shift per half; reading wm_box / wm_shift per half here costs the four-slot consumer registers it does not have (wm_plan keeps Cin = 32 to two slots per consumer)
+      const int row = ((NTW <= 2 && p.Cin == 32) ? p.wm_shift[g][tbeg + t][w >> 1] : p.wm_shift[g][tbeg + t][0]) + 2 * tq + h;
+      const int box = (NTW <= 2 && p.Cin == 32) ? 0 : (HALO ? 0 : 2 * (tbeg + t)) + (w >> 1);
+      off[t][h] = box * G::kXBox + row * 128 + ((((c >> 2) ^ row) & 7) << 4) + (c & 3) * 4;
     }
   }
   float acc[NTW][BN / 2];
@@ -283,16 +303,17 @@ __device__ __forceinline__ void wm_consume(const WgParams& p, const uint8_t* sme
 #pragma unroll
     for (int t = 0; t < NTW; ++t)
 #pragma unroll
-      for (int e = 0; e < 4; ++e) f[t][e] = __float_as_uint(cd_round_tf32(*reinterpret_cast<const float*>(xs + off[t][e] + kofs)));
+      for (int e = 0; e < 4; ++e)        // ci + 8 (odd e): 16-byte chunk index + 2, as c >> 2 has bit 1 clear
+        f[t][e] = __float_as_uint(cd_round_tf32(*reinterpret_cast<const float*>(xs + (off[t][e >> 1] ^ ((e & 1) * 32)) + kofs)));
   };
   if (nchunks == 0) return;
   mbar_wait(&afull[0], 0);
-  load_frags(fr[0], smem, 0);
+  load_frags(fr[0], smem + T::kRawBytes + T::kBBytes, 0);
   for (int it = 0; it < nchunks; ++it) {
     const uint32_t s = it % stages, ph = (it / stages) & 1u;
     mbar_wait(&bfull[s], ph);
-    const uint8_t* xs = smem + s * stage_bytes;
-    const uint32_t bs = smem_u32(xs + G::kXBytes + T::kRawBytes);
+    const uint8_t* xs = smem + s * stage_bytes + T::kRawBytes + T::kBBytes;
+    const uint32_t bs = smem_u32(smem + s * stage_bytes + T::kRawBytes);
 #pragma unroll
     for (int ks = 0; ks < kWmKR / 8; ++ks) {
       wgmma_fence();
@@ -307,17 +328,23 @@ __device__ __forceinline__ void wm_consume(const WgParams& p, const uint8_t* sme
       } else if (it + 1 < nchunks) {
         const uint32_t s1 = (it + 1) % stages, ph1 = ((it + 1) / stages) & 1u;
         mbar_wait(&afull[s1], ph1);
-        load_frags(fr[0], smem + s1 * stage_bytes, 0);
+        load_frags(fr[0], smem + s1 * stage_bytes + T::kRawBytes + T::kBBytes, 0);
       }
       wgmma_wait<0>();
     }
     __syncwarp();                      // every MMA of the chunk has retired: its X boxes and transposed tile are free
     if (lane == 0) { mbar_arrive(&aempty[s]); mbar_arrive(&bempty[s]); }
   }
-  // accumulator element (row, col) = (ci, co): rows 16 w + gq (+ 8), columns 8 j + 2 tq (+ 1)
+  // accumulator element (row, col) = (ci, co): rows 16 w + gq (+ 8), columns 8 j + 2 tq (+ 1); rows 32 h .. 32 h + 31 are the
+  // 32 channels of box wm_box[..][h].  Per-batch weights: image n = split / splits_per_img writes its own slice.
+  asm volatile("" ::: "memory");      // keeps the epilogue's parameter reads (and their registers) out of the main loop
+  const long long dw_off = p.per_batch ? (blockIdx.y / p.splits_per_img) * p.dw_batch_stride : 0;
 #pragma unroll
   for (int t = 0; t < NTW; ++t) {
-    float* wt = p.dw + static_cast<long long>(p.tap_index[g][tbeg + t]) * p.Cout * p.Cin + ci0 + 16 * w + gq;
+    const int tap = p.wm_tap[g][tbeg + t][w >> 1];
+    if (tap < 0) continue;
+    float* wt = p.dw + dw_off + static_cast<long long>(tap) * p.Cout * p.Cin + ci0 + 32 * p.wm_box[g][tbeg + t][w >> 1] +
+                16 * (w & 1) + gq;
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
@@ -328,13 +355,13 @@ __device__ __forceinline__ void wm_consume(const WgParams& p, const uint8_t* sme
   }
 }
 
-template <int BN, int NT, int CW>
+template <int BN, int NT, int CW, bool HALO>
 __global__ void __launch_bounds__(kWmThreads, 1)
 wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_constant__ CUtensorMap mapX, const __grid_constant__ WgParams p,
                    int stages) {
-  using G = WmGeom<CW>;
+  using G = WmGeom<CW, HALO>;
   using T = WmTiles<BN>;
-  constexpr int kStage = G::kXBytes + T::kRawBytes + T::kBBytes;
+  constexpr int kStage = WmStage<BN, CW, HALO>::kBytes;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
@@ -346,8 +373,8 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_const
   uint64_t* bfull = bars + 4 * stages;          // transposed tile written
   uint64_t* bempty = bars + 5 * stages;         // consumers done with the transposed tile
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
-  const int g = blockIdx.z, nt = p.ntaps[g];
-  const int ncons = nt > NT ? 2 : 1;            // consumer warpgroups with taps
+  const int g = blockIdx.z, nt = p.ntaps[g];    // accumulator slots of the group: ceil(nt / 2) in consumer 0, the rest in 1
+  const int ncons = nt > 1 ? 2 : 1;             // consumer warpgroups with slots
   if (threadIdx.x == 0) {
     for (int i = 0; i < stages; ++i) {
       mbar_init(&afull[i], 1); mbar_init(&aempty[i], 4 * ncons);
@@ -359,9 +386,15 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_const
   __syncthreads();
 
   const int tile = blockIdx.x;
-  const int co0 = (tile % p.tiles_co) * BN, ci0 = (tile / p.tiles_co) * 64;
-  const int c_beg = blockIdx.y * p.chunks_per_split;
+  const int co0 = (tile % p.tiles_co) * BN, ci0 = (tile / p.tiles_co) * p.ci_tile;
+  int c_beg = blockIdx.y * p.chunks_per_split;
   int c_end = c_beg + p.chunks_per_split; if (c_end > p.total_chunks) c_end = p.total_chunks;
+  if (p.per_batch) {                            // per-batch weights: splits never cross images
+    const int n = blockIdx.y / p.splits_per_img, sp = blockIdx.y % p.splits_per_img;
+    c_beg = n * p.chunks_per_img + sp * p.chunks_per_split;
+    c_end = c_beg + p.chunks_per_split;
+    if (c_end > (n + 1) * p.chunks_per_img) c_end = (n + 1) * p.chunks_per_img;
+  }
   const int nchunks = c_end > c_beg ? c_end - c_beg : 0;
 
   if (wg == 0) {
@@ -378,14 +411,15 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_const
         mbar_expect_tx(&rfull[s], T::kRawBytes);
 #pragma unroll
         for (int b = 0; b < BN / 32; ++b)
-          tma_load_4d(sx + G::kXBytes + b * T::kRawBox, &mapDY, &rfull[s], co0 + 32 * b, gx0, gy0, n);
+          tma_load_4d(sx + b * T::kRawBox, &mapDY, &rfull[s], co0 + 32 * b, gx0, gy0, n);
       }
       __syncwarp();
       mbar_wait(&aempty[s], ph ^ 1u);
       if (elect_one()) {
-        mbar_expect_tx(&afull[s], G::kXBytes);
-        tma_load_4d(sx, &mapX, &afull[s], ci0, gx0 - 1, gy0 - 1, n);
-        tma_load_4d(sx + G::kXBox, &mapX, &afull[s], ci0 + 32, gx0 - 1, gy0 - 1, n);
+        const int nb = p.wm_nbox[g], h = HALO ? 1 : 0;
+        mbar_expect_tx(&afull[s], nb * G::kXBox);
+        for (int b = 0; b < nb; ++b)
+          tma_load_4d(sx + T::kRawBytes + T::kBBytes + b * G::kXBox, &mapX, &afull[s], ci0 + 32 * b, gx0 - h, gy0 - h, n);
       }
       __syncwarp();
     }
@@ -399,8 +433,8 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_const
       const uint32_t s = it % stages, ph = (it / stages) & 1u;
       mbar_wait(&rfull[s], ph);
       mbar_wait(&bempty[s], ph ^ 1u);
-      const uint8_t* raw = smem + s * kStage + G::kXBytes;
-      uint8_t* bt = smem + s * kStage + G::kXBytes + T::kRawBytes;
+      const uint8_t* raw = smem + s * kStage;
+      uint8_t* bt = smem + s * kStage + T::kRawBytes;
       // unit u = (co box b, K quad kq): lane = co; K positions 4 kq .. 4 kq + 3 hold pixels 8 (kq / 2) + (kq & 1) + 2 j
 #pragma unroll 4
       for (int u = w4; u < (BN / 32) * (kWmKR / 4); u += 4) {
@@ -422,19 +456,22 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_const
     return;
   }
   // ===================== consumers =====================
-  const int tbeg = (wg - 2) * NT;
-  const int ntw = nt - tbeg < NT ? nt - tbeg : NT;
+  const int half = (nt + 1) / 2;
+  const int tbeg = (wg - 2) * half;
+  const int ntw = wg == 2 ? half : nt - half;
   if (ntw <= 0) return;
   asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(kWmRegsHigh));
-  if constexpr (NT == 4) {
-    if (ntw == 4) wm_consume<BN, 4, CW>(p, smem, stages, kStage, afull, aempty, bfull, bempty, nchunks, g, tbeg, co0, ci0);
-    else if (ntw == 3) wm_consume<BN, 3, CW>(p, smem, stages, kStage, afull, aempty, bfull, bempty, nchunks, g, tbeg, co0, ci0);
-    else if (ntw == 2) wm_consume<BN, 2, CW>(p, smem, stages, kStage, afull, aempty, bfull, bempty, nchunks, g, tbeg, co0, ci0);
-    else wm_consume<BN, 1, CW>(p, smem, stages, kStage, afull, aempty, bfull, bempty, nchunks, g, tbeg, co0, ci0);
+#define WM_CONSUME(n) wm_consume<BN, n, CW, HALO>(p, smem, stages, kStage, afull, aempty, bfull, bempty, nchunks, g, tbeg, co0, ci0)
+  if constexpr (NT == 4 && HALO) {        // 1x1: at most two slots per consumer
+    if (ntw == 4) WM_CONSUME(4);
+    else if (ntw == 3) WM_CONSUME(3);
+    else if (ntw == 2) WM_CONSUME(2);
+    else WM_CONSUME(1);
   } else {
-    if (ntw == 2) wm_consume<BN, 2, CW>(p, smem, stages, kStage, afull, aempty, bfull, bempty, nchunks, g, tbeg, co0, ci0);
-    else wm_consume<BN, 1, CW>(p, smem, stages, kStage, afull, aempty, bfull, bempty, nchunks, g, tbeg, co0, ci0);
+    if (ntw == 2) WM_CONSUME(2);
+    else WM_CONSUME(1);
   }
+#undef WM_CONSUME
 }
 
 int g_wg_mode = 1;      // 0: one X tile per tap (mma.sync); 8: mma.sync halo kernel; otherwise (default) the wgmma kernel where eligible
@@ -489,16 +526,17 @@ static int choose_splits(int tg, int total_chunks, int max_splits, int sms, doub
   return s;
 }
 
-template <int BN, int NT, int CW>
+constexpr int kWmSmem = 224 * 1024 + 1024 + 256;     // stages + 1024-byte alignment slack + barrier block
+
+template <int BN, int NT, int CW, bool HALO>
 static int launch_wm(dim3 grid, cudaStream_t st, const CUtensorMap& mapDY, const CUtensorMap& mapX, const WgParams& p) {
-  constexpr int kStage = WmGeom<CW>::kXBytes + WmTiles<BN>::kRawBytes + WmTiles<BN>::kBBytes;
+  constexpr int kStage = WmStage<BN, CW, HALO>::kBytes;
   int stages = (224 * 1024) / kStage; if (stages > 5) stages = 5;     // six barriers per stage in the 256-byte barrier block
-  static_assert((224 * 1024) / kStage >= 2, "two stages of the wgmma weight-gradient kernel fit shared memory");
   const size_t smem = size_t(stages) * kStage + 1024 + 256;
-  auto kern = wgrad_wgmma_kernel<BN, NT, CW>;
+  auto kern = wgrad_wgmma_kernel<BN, NT, CW, HALO>;
   static bool attr_done = false;
   if (!attr_done) {
-    CD_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CD_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kWmSmem));
     attr_done = true;
   }
   kern<<<grid, kWmThreads, smem, st>>>(mapDY, mapX, p, stages);
@@ -506,68 +544,139 @@ static int launch_wm(dim3 grid, cudaStream_t st, const CUtensorMap& mapDY, const
   return 0;
 }
 
-// wgmma kernel (see wgrad_wgmma_kernel); returns 1 when the problem is not eligible: it needs stride 1, a dense output map, taps
-// in [-1, 1]^2 (more than one), one weight set, Cin % 64 == 0, Cout % 64 == 0 and at least 64 pixels per image
+// NHWC tensor map {C, W, H, B} over the pixels (ey + sy i, ex + sx j) of a W0 x H0 image: dims W x H, box {32, bw, bh, 1}
+static int encode_nhwc(EncodeTiledFn enc, CUtensorMap* m, const float* base, int ld, int C, int W0, int H0, int B, int sy, int sx,
+                        int ey, int ex, int W, int H, int bw, int bh, const char* what) {
+  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+  cuuint64_t strides[3] = {(cuuint64_t)ld * 4 * sx, (cuuint64_t)ld * 4 * W0 * sy, (cuuint64_t)ld * 4 * W0 * H0};
+  cuuint32_t box[4] = {32, (cuuint32_t)bw, (cuuint32_t)bh, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  float* p = const_cast<float*>(base) + (static_cast<long long>(ey) * W0 + ex) * ld;
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r);
+  return 0;
+}
+
+// The stride-1 problem of one input-parity class: X pixel (ey + 2 (g + sy), ex + 2 (g + sx)) for the 4x4 stride-2 downsample,
+// X pixel g + (sy, sx) otherwise.  Builds the accumulator slots and groups; returns 1 when they do not fit the kernel.
+struct WmClass { int ey, ex, n, tap[16], sy[16], sx[16]; };
+
+static int wm_plan(const CdConvDesc* d, const WmClass& k, int BN, int CW, WgParams& p, bool& halo) {
+  const int Cin = d->s[0].C, NT = BN == 128 ? 2 : 4;
+  halo = !(k.n == 1 && k.sy[0] == 0 && k.sx[0] == 0);
+  p.tiles_co = d->Cout / BN;
+  // slots: [half 0 | half 1] = (box, row shift, tap)
+  int sb[16][2], ss[16][2], st[16][2], ns = 0, nbox = 2;
+  auto shift = [&](int i) { return halo ? (k.sy[i] + 1) * (CW + 8) + k.sx[i] + 1 : 0; };
+  if (Cin == 32) {              // image edge: one 32-ci box; the two halves of a slot take two taps
+    if (halo && BN != 128) return 1;
+    nbox = 1;
+    for (int i = 0; i < k.n; i += 2, ++ns)
+      for (int h = 0; h < 2; ++h) {
+        const bool on = i + h < k.n;
+        sb[ns][h] = 0; ss[ns][h] = on ? shift(i + h) : 0; st[ns][h] = on ? k.tap[i + h] : -1;
+      }
+  } else if (!halo) {
+    // 1x1: the slots of a CTA are consecutive 64-ci blocks sharing one transposed dY tile: the most that divides Cin / 64
+    ns = wm_slots_1x1(BN);
+    while ((Cin / 64) % ns != 0) --ns;
+    nbox = 2 * ns;
+    for (int t = 0; t < ns; ++t)
+      for (int h = 0; h < 2; ++h) { sb[t][h] = 2 * t + h; ss[t][h] = 0; st[t][h] = k.tap[0]; }
+  } else {                      // one tap per slot, both halves from the two 32-ci boxes of the CTA's 64 ci
+    for (int i = 0; i < k.n; ++i, ++ns)
+      for (int h = 0; h < 2; ++h) { sb[ns][h] = h; ss[ns][h] = shift(i); st[ns][h] = k.tap[i]; }
+  }
+  p.ci_tile = Cin == 32 ? 32 : 32 * nbox;
+  p.tiles_ci = Cin == 32 ? 1 : Cin / p.ci_tile;
+  p.ngroups = cd_cdiv(ns, 2 * NT);           // tap groups on grid z (9 taps: {4, 4, 1} or {8, 1})
+  if (p.ngroups > kMaxGroups) return 1;
+  for (int g = 0; g < p.ngroups; ++g) {
+    const int s0 = g * 2 * NT, n = ns - s0 < 2 * NT ? ns - s0 : 2 * NT;
+    p.ntaps[g] = n;
+    p.wm_nbox[g] = nbox;
+    for (int t = 0; t < n; ++t)
+      for (int h = 0; h < 2; ++h) { p.wm_box[g][t][h] = sb[s0 + t][h]; p.wm_shift[g][t][h] = ss[s0 + t][h]; p.wm_tap[g][t][h] = st[s0 + t][h]; }
+  }
+  return 0;
+}
+
+// wgmma kernel (see wgrad_wgmma_kernel); returns 1 when the problem is not eligible.  It takes stride-1 problems with taps in
+// [-1, 1]^2 (3x3, 1x1, the four taps of a transposed-convolution parity class, whose dY is read at every second pixel) and the
+// 4x4 stride-2 downsample, split into its four input-parity classes of four stride-1 taps each (one launch per class, X read at
+// every second pixel).  Cin % 64 == 0 or Cin == 32 (image edge), Cout % 64 == 0, per-batch weights allowed.
 static int wgrad_wgmma(const CdConvDesc* d, const float* dout, int dout_ld, float* dw, EncodeTiledFn enc, cudaStream_t st) {
   const CdConvSrc& c = d->s[0];
-  if (c.w_per_batch || d->sy != 1 || d->sx != 1 || d->oys != 1 || d->oxs != 1 || d->oy0 != 0 || d->ox0 != 0) return 1;
-  if (c.H != d->Hg || c.W != d->Wg || d->Ho != d->Hg || d->Wo != d->Wg) return 1;
-  if (c.C % 64 != 0 || d->Cout % 64 != 0 || c.ntaps < 2 || c.ntaps > 9) return 1;
-  for (int t = 0; t < c.ntaps; ++t) if (c.dy[t] < -1 || c.dy[t] > 1 || c.dx[t] < -1 || c.dx[t] > 1) return 1;
+  if ((c.C % 64 != 0 && c.C != 32) || d->Cout % 64 != 0 || c.ntaps < 1) return 1;
+  const bool dense_out = d->oys == 1 && d->oxs == 1 && d->oy0 == 0 && d->ox0 == 0 && d->Ho == d->Hg && d->Wo == d->Wg;
+  const bool parity_out = d->oys == 2 && d->oxs == 2 && (d->oy0 & ~1) == 0 && (d->ox0 & ~1) == 0 && d->Ho == 2 * d->Hg &&
+                          d->Wo == 2 * d->Wg;
+  const bool s1 = d->sy == 1 && d->sx == 1 && c.H == d->Hg && c.W == d->Wg && (dense_out || parity_out);
+  const bool s2 = d->sy == 2 && d->sx == 2 && c.H == 2 * d->Hg && c.W == 2 * d->Wg && dense_out;
+  if (!s1 && !s2) return 1;
   const int CW = d->Wg >= 16 ? 16 : 8, R = kWmKR / CW;
   if (d->Hg < R) return 1;
   const int BN = d->Cout % 128 == 0 ? 128 : 64;
-  const int NT = BN == 128 ? 2 : 4;              // taps per consumer warpgroup: 128 accumulator registers
-  WgParams p{};
-  p.B = d->B; p.Hg = d->Hg; p.Wg = d->Wg; p.Cout = d->Cout; p.Cin = c.C;
-  p.sy = 1; p.sx = 1; p.oys = 1; p.oxs = 1;
-  p.dw = dw;
-  p.CW = CW; p.R = R; p.KR = kWmKR;
-  // tap groups of up to 2 NT taps on grid z; the last one takes the remainder (9 taps: {4, 4, 1} or {8, 1})
-  p.ngroups = cd_cdiv(c.ntaps, 2 * NT);
-  for (int gk = 0; gk < p.ngroups; ++gk) {
-    const int t0 = gk * 2 * NT, n = c.ntaps - t0 < 2 * NT ? c.ntaps - t0 : 2 * NT;
-    p.ntaps[gk] = n;
-    for (int k = 0; k < n; ++k) {
-      p.tap_index[gk][k] = t0 + k;
-      p.tap_shift[gk][k] = (c.dy[t0 + k] + 1) * (CW + 8) + c.dx[t0 + k] + 1;
+  WmClass cls[4];
+  int ncls = 0;
+  for (int e = 0; e < (s2 ? 4 : 1); ++e) {
+    WmClass& k = cls[ncls];
+    k.ey = e >> 1; k.ex = e & 1; k.n = 0;
+    for (int t = 0; t < c.ntaps; ++t) {
+      if (s2 && ((c.dy[t] & 1) != k.ey || (c.dx[t] & 1) != k.ex)) continue;
+      const int sy = s2 ? (c.dy[t] - k.ey) / 2 : c.dy[t], sx = s2 ? (c.dx[t] - k.ex) / 2 : c.dx[t];
+      if (sy < -1 || sy > 1 || sx < -1 || sx > 1) return 1;
+      k.tap[k.n] = t; k.sy[k.n] = sy; k.sx[k.n] = sx; ++k.n;
     }
+    if (k.n > 0) ++ncls;
   }
-  p.chunks_x = d->Wg / CW; p.chunks_y = d->Hg / R;
-  p.total_chunks = d->B * p.chunks_x * p.chunks_y;
-  p.tiles_co = d->Cout / BN; p.tiles_ci = c.C / 64;
-  const int tiles = p.tiles_co * p.tiles_ci;
-  // MMAs of one chunk: the busier warpgroup's taps x 8 k-steps of m64nBNk8, at the wgmma TF32 rate of 2048 FLOP/clk per SM
-  // shared by both warpgroups
-  const int max_taps = p.ntaps[0];
-  const double chunk_clk = double(max_taps) * (kWmKR / 8) * (BN / 2);
-  const int splits = choose_splits(tiles * p.ngroups, p.total_chunks, cd_cdiv(p.total_chunks, 8), g_sms, chunk_clk);
-  p.chunks_per_split = cd_cdiv(p.total_chunks, splits);
-  p.splits = cd_cdiv(p.total_chunks, p.chunks_per_split);
-
-  CUtensorMap mapDY, mapX;
-  const CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;   // both operands are rounded RN to TF32 in the kernel
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)d->Cout, (cuuint64_t)d->Wo, (cuuint64_t)d->Ho, (cuuint64_t)d->B};
-    cuuint64_t strides[3] = {(cuuint64_t)dout_ld * 4, (cuuint64_t)dout_ld * 4 * d->Wo, (cuuint64_t)dout_ld * 4 * d->Wo * d->Ho};
-    cuuint32_t box[4] = {32, (cuuint32_t)CW, (cuuint32_t)R, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&mapDY, dt, 4, const_cast<float*>(dout), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(wgmma dY) failed: %d", (int)r);
+  // every class is checked before the first launch
+  WgParams ps[4];
+  bool halo[4];
+  for (int i = 0; i < ncls; ++i) {
+    ps[i] = WgParams{};
+    if (wm_plan(d, cls[i], BN, CW, ps[i], halo[i])) return 1;
   }
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)c.C, (cuuint64_t)c.W, (cuuint64_t)c.H, (cuuint64_t)d->B};
-    cuuint64_t strides[3] = {(cuuint64_t)c.ld * 4, (cuuint64_t)c.ld * 4 * c.W, (cuuint64_t)c.ld * 4 * c.W * c.H};
-    cuuint32_t box[4] = {32, (cuuint32_t)(CW + 8), (cuuint32_t)(R + 2), 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&mapX, dt, 4, const_cast<float*>(c.src), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(wgmma X) failed: %d", (int)r);
+  CUtensorMap mapDY;
+  if (encode_nhwc(enc, &mapDY, dout, dout_ld, d->Cout, d->Wo, d->Ho, d->B, d->oys, d->oxs, d->oy0, d->ox0, d->Wg, d->Hg, CW, R, "wgmma dY")) return -1;
+  for (int i = 0; i < ncls; ++i) {
+    WgParams& p = ps[i];
+    p.B = d->B; p.Hg = d->Hg; p.Wg = d->Wg; p.Cout = d->Cout; p.Cin = c.C;
+    p.dw = dw;
+    p.CW = CW; p.R = R; p.KR = kWmKR;
+    p.chunks_x = d->Wg / CW; p.chunks_y = d->Hg / R;
+    p.total_chunks = d->B * p.chunks_x * p.chunks_y;
+    const int tiles = p.tiles_co * p.tiles_ci;
+    // MMAs of one chunk: the group's slots x 8 k-steps of m64nBNk8, at the wgmma TF32 rate of 2048 FLOP/clk per SM shared by both
+    // consumer warpgroups
+    const double chunk_clk = double(p.ntaps[0]) * (kWmKR / 8) * (BN / 2);
+    if (c.w_per_batch) {
+      p.per_batch = 1;
+      p.chunks_per_img = p.chunks_x * p.chunks_y;
+      const int spi = choose_splits(tiles * p.ngroups * d->B, p.chunks_per_img, p.chunks_per_img, g_sms, chunk_clk);
+      p.chunks_per_split = cd_cdiv(p.chunks_per_img, spi);
+      p.splits_per_img = cd_cdiv(p.chunks_per_img, p.chunks_per_split);
+      p.splits = p.splits_per_img * d->B;
+      p.dw_batch_stride = static_cast<long long>(c.ntaps) * d->Cout * c.C;
+    } else {
+      const int splits = choose_splits(tiles * p.ngroups, p.total_chunks, cd_cdiv(p.total_chunks, 8), g_sms, chunk_clk);
+      p.chunks_per_split = cd_cdiv(p.total_chunks, splits);
+      p.splits = cd_cdiv(p.total_chunks, p.chunks_per_split);
+    }
+    CUtensorMap mapX;
+    const int bw = halo[i] ? CW + 8 : CW, bh = halo[i] ? R + 2 : R;
+    if (encode_nhwc(enc, &mapX, c.src, c.ld, c.C, c.W, c.H, d->B, d->sy, d->sx, cls[i].ey, cls[i].ex, d->Wg, d->Hg, bw, bh, "wgmma X")) return -1;
+    const dim3 grid(tiles, p.splits, p.ngroups);
+#define WM_LAUNCH(bn, nt, cw) (halo[i] ? launch_wm<bn, nt, cw, true>(grid, st, mapDY, mapX, p) \
+                                       : launch_wm<bn, nt, cw, false>(grid, st, mapDY, mapX, p))
+    int rc;
+    if (BN == 128) rc = CW == 16 ? WM_LAUNCH(128, 2, 16) : WM_LAUNCH(128, 2, 8);
+    else rc = CW == 16 ? WM_LAUNCH(64, 4, 16) : WM_LAUNCH(64, 4, 8);
+#undef WM_LAUNCH
+    if (rc) return rc;
   }
-  const dim3 grid(tiles, p.splits, p.ngroups);
-  if (BN == 128) return CW == 16 ? launch_wm<128, 2, 16>(grid, st, mapDY, mapX, p) : launch_wm<128, 2, 8>(grid, st, mapDY, mapX, p);
-  return CW == 16 ? launch_wm<64, 4, 16>(grid, st, mapDY, mapX, p) : launch_wm<64, 4, 8>(grid, st, mapDY, mapX, p);
+  return 0;
 }
 
 // returns 1 if the problem is not tensor-core shaped (caller falls back to the SIMT kernel), 0 on success, <0 on error

@@ -297,7 +297,14 @@ class BackwardMixin:
         dweff.zero_()
         qv = View(qkv, 0, 128)
         d = ops.make_conv_desc([(qv, T1, dweff, True)], dyv, grid, Cout=dim)
-        ops.conv_wgrad(d, dyv, dweff, None, impl=self.conv_impl)
+        if self.profile_wgrads is not None:                 # tools/wgrad_shapes.py: stride column 'batch' marks per-batch weights
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            ops.conv_wgrad(d, dyv, dweff, None, impl=self.conv_impl)
+            e1.record()
+            self.profile_wgrads.append((e0, e1, (B, H, W, dim, 128, 1, 'batch')))
+        else:
+            ops.conv_wgrad(d, dyv, dweff, None, impl=self.conv_impl)
         dctxn = self.buf('g.dctxn', (B, 4, 32, 32))
         rowdot = self.buf('g.rowdot', (B, 128))
         call('cd_linattn_bwd_small', ptr(dweff), ptr(ctx), ptr(ksum), ptr(a.to_out.weight), B, dim, C.c_float(a.scale),

@@ -10,7 +10,8 @@ the kernel choices and K-split policies of csrc/wgrad_tc.cu (cd_wgrad_tc_set_mod
 The configurations are taken in turns, so that clock drift under the power cap hits them all alike.  Per shape it prints
 microseconds per launch and achieved TFLOP/s of each configuration, and for the 3x3 shapes the modelled shared-memory bytes per
 FLOP of each kernel (the mainloop's shared-memory traffic: operand loads, TMA writes, the dY transposition; bank conflicts
-counted as extra wavefronts), then the totals per backward: all shapes and the 3x3 shapes alone."""
+counted as extra wavefronts), then the totals per backward: all shapes, the 3x3 shapes alone and the rest.  The per-batch
+attention product dweff is listed with stride 'batch'."""
 import sys, io, contextlib, os, collections
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -111,6 +112,7 @@ for shp in res[names[0]]:
     model = ("%12.3f" % mw if mw else "%12s" % '-') + ("%9.3f" % ms_ if ms_ else "%9s" % '-')
     print("%-34s %3d " % (str(shp), n) + " ".join("%10.1f" % v for v in us) + "  " + " ".join("%9.1f" % v for v in tf) + model)
 print("%-34s     " % "total ms per backward" + " ".join("%10.3f" % tot[n] for n in names))
+print("%-34s     " % "other shapes ms per backward" + " ".join("%10.3f" % (tot[n] - tot3[n]) for n in names))
 print("%-34s     " % "3x3 (stride 1) ms per backward" + " ".join("%10.3f" % tot3[n] for n in names))
 if len(names) > 1 and tot3[names[0]] > 0:
     print("3x3 total, %s / %s: %.2fx" % (names[1], names[0], tot3[names[1]] / tot3[names[0]]))
