@@ -479,7 +479,8 @@ def test_depthwise_kernels_with_tma_staged_tiles_match_the_ldgsts_kernels_and_to
     import torch.nn.functional as F
     from cold_diffusion_models_b200._lib import lib, ptr, stream, _check
     gen = torch.Generator().manual_seed(11)
-    for (B, H, W, Cc, pad) in ((2, 32, 32, 64, 0), (3, 16, 48, 32, 4), (1, 128, 128, 64, 0), (2, 16, 16, 96, 32)):
+    for (B, H, W, Cc, pad) in ((2, 32, 32, 64, 0), (3, 16, 48, 32, 4), (1, 128, 128, 64, 0), (2, 16, 16, 96, 32),
+                               (32, 64, 64, 128, 0), (32, 32, 32, 256, 0), (32, 16, 16, 512, 0)):     # the config-3 levels at B = 32
         ld = Cc + pad
         x = torch.randn(B, H, W, ld, generator=gen).cuda()
         dh = torch.randn(B, H, W, ld, generator=gen).cuda()
