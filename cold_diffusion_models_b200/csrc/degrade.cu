@@ -170,6 +170,241 @@ blur_step_down_kernel(const float* __restrict__ xt, const float* __restrict__ xh
   }
 }
 
+// ---- 128 < S <= 512: one CTA per (plane, strip of kStripR rows) ----------------------------------------------------------
+// A plane, its operator and the intermediate no longer fit in shared memory, but a row strip of Z = A X A^T needs only the
+// same rows of A:  Z[r0:r0+R, :] = (A[r0:r0+R, :] X) A^T.
+//   phase 1: Y = A[r0:r0+R, :] X  (R x S), kept in shared memory transposed (Yt[k][r]);
+//   phase 2: Z_strip[r][j] = sum_k Y[r][k] A[j][k].
+// X (phase 1) and A^T (phase 2) stream through a double-buffered ring of kStripK-row chunks (cp.async; the A^T chunk is
+// transposed by 4-byte copies), so the intermediate never reaches HBM and X / A_t are re-read from L2 once per strip; the
+// strips of one plane are adjacent in the grid.  Warp w owns the strip rows 4w..4w+3, lane l the columns 4l + 128q
+// (q < NQ = ceil(S / 128)): 16 NQ fp32 FFMA accumulators per thread.  When S is not a multiple of 128 the ring columns
+// S .. 128 NQ - 1 are never written: they feed only the accumulators of columns j >= S, which are never stored (neither to Yt
+// nor to the output), so whatever they hold does not reach a result.  The caller must not alias out with x / xhat: the
+// other strips of a plane still read it.
+constexpr int kStripR = 32, kStripK = 16, kStripThreads = 256, kStripLdy = kStripR + 4;
+
+template <int NQ> __host__ __device__ constexpr int strip_ldb() { return 128 * NQ + 4; }
+__host__ __device__ __forceinline__ int strip_cdiv(int a, int b) { return (a + b - 1) / b; }
+
+// floats of shared memory: ring 2 x [kStripK][ldb] | A-strip ring 2 x [kStripK][kStripR] | Yt [S rounded up to kStripK][kStripLdy]
+// | scratch 32  (the plane-mean path keeps its column sums w[S] where Yt goes)
+template <int NQ> size_t strip_smem(int S) {
+  return sizeof(float) * (2 * kStripK * strip_ldb<NQ>() + 2 * kStripK * kStripR + size_t(strip_cdiv(S, kStripK)) * kStripK * kStripLdy + 32);
+}
+
+__device__ __forceinline__ void fma4x4(float (&acc)[4][4], float4 a, float4 b) {
+  const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+}
+
+// f(q, a, offset of Z[r][j] in the plane) for every in-plane float4 this thread owns: r = r0 + 4w + a, j = 4 lane + 128 q
+template <int NQ, typename F>
+__device__ __forceinline__ void strip_for_each(int S, int r0, F f) {
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int q = 0; q < NQ; ++q)
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+      const int r = r0 + 4 * w + a, j = 4 * lane + 128 * q;
+      if (r < S && j < S) f(q, a, static_cast<long long>(r) * S + j);
+    }
+}
+
+// acc <- this thread's part of the strip of A X A^T (rows and columns outside the plane hold garbage)
+template <int NQ>
+__device__ __forceinline__ void strip_product(const float* __restrict__ A, const float* __restrict__ X, int S, int r0, float* sm,
+                                              float (&acc)[NQ][4][4]) {
+  constexpr int ldb = strip_ldb<NQ>();
+  float* ring = sm;
+  float* aring = ring + 2 * kStripK * ldb;
+  float* Yt = aring + 2 * kStripK * kStripR;
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nk = strip_cdiv(S, kStripK), per_row = S >> 2;
+  auto zero = [&] {
+#pragma unroll
+    for (int q = 0; q < NQ; ++q)
+#pragma unroll
+      for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b) acc[q][a][b] = 0.f;
+  };
+  // chunk c: `issue` fills ring buffer c & 1 and commits, then every chunk is waited for, consumed by `compute` and released
+  auto run = [&](auto issue, auto compute) {
+    issue(0);
+    for (int c = 0; c < nk; ++c) {
+      if (c + 1 < nk) {
+        issue(c + 1);
+        asm volatile("cp.async.wait_group 1;" ::: "memory");
+      } else {
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+      }
+      __syncthreads();
+      compute(c);
+      __syncthreads();
+    }
+  };
+  // phase 1, chunk c: ring[kk][j] = X[k0 + kk][j], aring[kk][r] = A[r0 + r][k0 + kk]  (zero outside the plane)
+  auto issue1 = [&](int c) {
+    const int k0 = c * kStripK;
+    float* rb = ring + (c & 1) * kStripK * ldb;
+    for (int i = threadIdx.x; i < kStripK * per_row; i += kStripThreads) {
+      const int kk = i / per_row, j = (i - kk * per_row) * 4;
+      const bool v = k0 + kk < S;
+      cd_cp_async16(rb + kk * ldb + j, X + (v ? static_cast<long long>(k0 + kk) * S + j : 0), v);
+    }
+    float* ab = aring + (c & 1) * kStripK * kStripR;
+    for (int i = threadIdx.x; i < kStripK * kStripR; i += kStripThreads) {
+      const int r = i / kStripK, kk = i - r * kStripK;          // kk fastest: a warp reads two 64-byte row segments of A
+      const bool v = r0 + r < S && k0 + kk < S;
+      cd_cp_async4(ab + kk * kStripR + r, A + (v ? static_cast<long long>(r0 + r) * S + k0 + kk : 0), v);
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  auto compute1 = [&](int c) {
+    const float* rb = ring + (c & 1) * kStripK * ldb + 4 * lane;
+    const float* ab = aring + (c & 1) * kStripK * kStripR + 4 * w;
+#pragma unroll 4
+    for (int kk = 0; kk < kStripK; ++kk) {
+      const float4 a = *reinterpret_cast<const float4*>(ab + kk * kStripR);
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) fma4x4(acc[q], a, *reinterpret_cast<const float4*>(rb + kk * ldb + 128 * q));
+    }
+  };
+  // phase 2, chunk c: ring[kk][j] = A[j][k0 + kk]
+  auto issue2 = [&](int c) {
+    const int k0 = c * kStripK;
+    float* rb = ring + (c & 1) * kStripK * ldb;
+    for (int i = threadIdx.x; i < kStripK * S; i += kStripThreads) {
+      const int j = i / kStripK, kk = i - j * kStripK;
+      const bool v = k0 + kk < S;
+      cd_cp_async4(rb + kk * ldb + j, A + (v ? static_cast<long long>(j) * S + k0 + kk : 0), v);
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  auto compute2 = [&](int c) {
+    const float* rb = ring + (c & 1) * kStripK * ldb + 4 * lane;
+    const float* yb = Yt + c * kStripK * kStripLdy + 4 * w;
+#pragma unroll 4
+    for (int kk = 0; kk < kStripK; ++kk) {
+      const float4 y = *reinterpret_cast<const float4*>(yb + kk * kStripLdy);
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) fma4x4(acc[q], y, *reinterpret_cast<const float4*>(rb + kk * ldb + 128 * q));
+    }
+  };
+  zero();
+  run(issue1, compute1);
+  // Yt[j][r] = Y[r][j]; the rows past S (the last chunk's tail) are zero, as is the A^T chunk there
+#pragma unroll
+  for (int q = 0; q < NQ; ++q)
+#pragma unroll
+    for (int b = 0; b < 4; ++b) {
+      const int j = 4 * lane + 128 * q + b;
+      if (j < S) *reinterpret_cast<float4*>(Yt + j * kStripLdy + 4 * w) = make_float4(acc[q][0][b], acc[q][1][b], acc[q][2][b], acc[q][3][b]);
+    }
+  for (int i = S * kStripLdy + threadIdx.x; i < nk * kStripK * kStripLdy; i += kStripThreads) Yt[i] = 0.f;
+  zero();
+  run(issue2, compute2);                  // its first barrier orders the Yt writes before any read
+}
+
+// mean(A X A^T) = w^T X w / S^2 with w = A^T 1 (column sums of A): the `discrete` collapse without the strip product
+__device__ __forceinline__ float plane_mean_closed_form(const float* __restrict__ A, const float* __restrict__ X, int S,
+                                                        float* w, float* scratch) {
+  for (int k = threadIdx.x; k < S; k += blockDim.x) {
+    float s = 0.f;
+    for (int j = 0; j < S; ++j) s += __ldg(A + static_cast<long long>(j) * S + k);
+    w[k] = s;
+  }
+  __syncthreads();
+  float s = 0.f;
+  for (int i = threadIdx.x; i < S * S; i += blockDim.x) s = fmaf(w[i / S] * __ldg(X + i), w[i % S], s);
+  return block_sum(s, scratch) / (static_cast<float>(S) * S);
+}
+
+// acc <- this thread's part of the strip of D = A_idx X A_idx^T  (idx < 0: X itself; collapse at idx == T-1: the plane mean)
+template <int NQ>
+__device__ __forceinline__ void strip_degrade(const float* __restrict__ ops, const float* __restrict__ X, int idx, int S, int T,
+                                              int collapse_last, int r0, float* sm, float (&acc)[NQ][4][4]) {
+  if (idx < 0) {
+    strip_for_each<NQ>(S, r0, [&](int q, int a, long long o) {
+      const float4 v = __ldg(reinterpret_cast<const float4*>(X + o));
+      acc[q][a][0] = v.x; acc[q][a][1] = v.y; acc[q][a][2] = v.z; acc[q][a][3] = v.w;
+    });
+    return;
+  }
+  const float* A = ops + static_cast<long long>(idx) * S * S;
+  if (collapse_last && idx == T - 1) {
+    float* w = sm + 2 * kStripK * strip_ldb<NQ>() + 2 * kStripK * kStripR;
+    const float mean = plane_mean_closed_form(A, X, S, w, w + strip_cdiv(S, kStripK) * kStripK * kStripLdy);
+#pragma unroll
+    for (int q = 0; q < NQ; ++q)
+#pragma unroll
+      for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b) acc[q][a][b] = mean;
+    return;
+  }
+  strip_product<NQ>(A, X, S, r0, sm, acc);
+}
+
+template <int NQ>
+__global__ void __launch_bounds__(kStripThreads, 1)
+blur_apply_strip_kernel(const float* __restrict__ x, float* __restrict__ out, const float* __restrict__ ops,
+                        const long long* __restrict__ t, int t_scalar, int C, int S, int T, int collapse_last, int quantize) {
+  extern __shared__ __align__(16) float sm[];
+  const int nstrip = strip_cdiv(S, kStripR);
+  const int pl = blockIdx.x / nstrip;                     // b * C + c; the strips of one plane are adjacent
+  const int r0 = (blockIdx.x - pl * nstrip) * kStripR;
+  const float* xp = x + static_cast<long long>(pl) * S * S;
+  float* op = out + static_cast<long long>(pl) * S * S;
+  const int idx = t ? static_cast<int>(t[pl / C]) : t_scalar;
+  float acc[NQ][4][4];
+  strip_degrade<NQ>(ops, xp, idx, S, T, collapse_last, r0, sm, acc);
+  strip_for_each<NQ>(S, r0, [&](int q, int a, long long o) {
+    float f[4] = {acc[q][a][0], acc[q][a][1], acc[q][a][2], acc[q][a][3]};
+    if (quantize) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {          // DB:954-958, same op order as blur_apply_kernel
+        float qv = (f[k] + 1.f) * 0.5f;
+        qv = qv * 255.f;
+        qv = static_cast<float>(static_cast<int>(qv)) / 255.f;
+        f[k] = qv * 2.f - 1.f;
+      }
+    }
+    *reinterpret_cast<float4*>(op + o) = make_float4(f[0], f[1], f[2], f[3]);
+  });
+}
+
+// out = xt - Z_hi + Z_lo: xt - Z_hi is parked in `out` and read back by the thread that wrote it
+template <int NQ>
+__global__ void __launch_bounds__(kStripThreads, 1)
+blur_step_down_strip_kernel(const float* __restrict__ xt, const float* __restrict__ xhat, float* out, const float* __restrict__ ops,
+                            int t_hi, int t_lo, int S, int T, int collapse_last) {
+  extern __shared__ __align__(16) float sm[];
+  const int nstrip = strip_cdiv(S, kStripR);
+  const int pl = blockIdx.x / nstrip;
+  const int r0 = (blockIdx.x - pl * nstrip) * kStripR;
+  const float* xh = xhat + static_cast<long long>(pl) * S * S;
+  const float* xp = xt + static_cast<long long>(pl) * S * S;
+  float* op = out + static_cast<long long>(pl) * S * S;
+  float acc[NQ][4][4];
+  strip_degrade<NQ>(ops, xh, t_hi, S, T, collapse_last, r0, sm, acc);
+  strip_for_each<NQ>(S, r0, [&](int q, int a, long long o) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(xp + o));
+    *reinterpret_cast<float4*>(op + o) = make_float4(v.x - acc[q][a][0], v.y - acc[q][a][1], v.z - acc[q][a][2], v.w - acc[q][a][3]);
+  });
+  __syncthreads();
+  strip_degrade<NQ>(ops, xh, t_lo, S, T, 0, r0, sm, acc);
+  strip_for_each<NQ>(S, r0, [&](int q, int a, long long o) {
+    float4 d = *reinterpret_cast<const float4*>(op + o);
+    d.x += acc[q][a][0]; d.y += acc[q][a][1]; d.z += acc[q][a][2]; d.w += acc[q][a][3];
+    *reinterpret_cast<float4*>(op + o) = d;
+  });
+}
+
 // ---- loss -----------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 loss_kernel(const float* __restrict__ x0, const float* __restrict__ xhat, long long n, int mode, float inv_n,
@@ -222,9 +457,51 @@ extern "C" int cd_ema_update(float* ema, const float* p, int64_t n, float beta, 
 
 static size_t blur_smem(int S, int planes) { return sizeof(float) * (size_t(S) * S + size_t(planes) * S * (S + 4) + 32); }
 
+// grid of the strip kernels: one CTA per (plane, strip), strips of a plane adjacent
+static int strip_grid(int B, int C, int S, unsigned* grid) {
+  const long long n = static_cast<long long>(B) * C * cd_cdiv(S, kStripR);
+  CD_REQUIRE(n >= 1 && n < (1ll << 31), "blur strip kernels: %lld CTAs out of range", n);
+  *grid = static_cast<unsigned>(n);
+  return 0;
+}
+
+template <int NQ>
+static int blur_apply_strips(const float* x, float* out, const float* ops, const int64_t* t, int t_scalar, int B, int C, int S,
+                             int T, int collapse_last, int quantize, cudaStream_t stream) {
+  unsigned grid = 0;
+  if (strip_grid(B, C, S, &grid)) return -1;
+  const size_t smem = strip_smem<NQ>(S);
+  static size_t attr = 0;
+  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_apply_strip_kernel<NQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
+  blur_apply_strip_kernel<NQ><<<grid, kStripThreads, smem, stream>>>(x, out, ops, reinterpret_cast<const long long*>(t), t_scalar,
+                                                                    C, S, T, collapse_last, quantize);
+  CD_LAUNCH_CHECK();
+  return 0;
+}
+
+template <int NQ>
+static int blur_step_down_strips(const float* xt, const float* xhat, float* out, const float* ops, int t_hi, int t_lo, int B, int C,
+                                 int S, int T, int collapse_last, cudaStream_t stream) {
+  unsigned grid = 0;
+  if (strip_grid(B, C, S, &grid)) return -1;
+  const size_t smem = strip_smem<NQ>(S);
+  static size_t attr = 0;
+  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_step_down_strip_kernel<NQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
+  blur_step_down_strip_kernel<NQ><<<grid, kStripThreads, smem, stream>>>(xt, xhat, out, ops, t_hi, t_lo, S, T, collapse_last);
+  CD_LAUNCH_CHECK();
+  return 0;
+}
+
+// S <= 128: one CTA per plane (blur_apply_kernel / blur_step_down_kernel); 128 < S <= 512: one CTA per row strip
 extern "C" int cd_blur_apply(const float* x, float* out, const float* ops, const int64_t* t, int t_scalar,
                              int B, int C, int S, int T, int collapse_last, int quantize, void* stream) {
-  CD_REQUIRE(S % 4 == 0 && S >= 4 && S <= 128, "cd_blur_apply: image size %d unsupported (need S%%4==0, S<=128)", S);
+  CD_REQUIRE(S % 4 == 0 && S >= 4 && S <= 512, "cd_blur_apply: image size %d unsupported (need S%%4==0, 4<=S<=512)", S);
+  if (S > 128) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (S <= 256) return blur_apply_strips<2>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, st);
+    if (S <= 384) return blur_apply_strips<3>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, st);
+    return blur_apply_strips<4>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, st);
+  }
   const size_t smem = blur_smem(S, 2);
   static size_t attr = 0;
   if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
@@ -237,7 +514,13 @@ extern "C" int cd_blur_apply(const float* x, float* out, const float* ops, const
 
 extern "C" int cd_blur_step_down(const float* xt, const float* xhat, float* out, const float* ops,
                                  int t_hi, int t_lo, int B, int C, int S, int T, int collapse_last, void* stream) {
-  CD_REQUIRE(S % 4 == 0 && S >= 4 && S <= 128, "cd_blur_step_down: image size %d unsupported", S);
+  CD_REQUIRE(S % 4 == 0 && S >= 4 && S <= 512, "cd_blur_step_down: image size %d unsupported (need S%%4==0, 4<=S<=512)", S);
+  if (S > 128) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (S <= 256) return blur_step_down_strips<2>(xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, collapse_last, st);
+    if (S <= 384) return blur_step_down_strips<3>(xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, collapse_last, st);
+    return blur_step_down_strips<4>(xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, collapse_last, st);
+  }
   const size_t smem = blur_smem(S, 2);
   static size_t attr = 0;
   if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_step_down_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }

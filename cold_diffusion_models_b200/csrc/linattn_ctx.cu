@@ -178,7 +178,12 @@ extern "C" int cd_linattn_context_det(const float* qkv, int ld, int B, int n, in
   if (!attr) { CD_CUDA(cudaFuncSetAttribute(ctx_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
   ctx_partial_kernel<<<dim3(nblk, B), 256, smem, st>>>(qkv, ld, n, ppb, ws);
   CD_LAUNCH_CHECK();
-  ctx_merge_kernel<<<dim3(4, B), 256, sizeof(float) * nblk * 32, st>>>(ws, nblk, kmax, ksum, ctx);
+  // the merge keeps 32 weights per span: above 384 spans (one 512^2 image at the finest level) that passes the 48 KB a launch
+  // gets without opting in
+  const size_t msmem = sizeof(float) * nblk * 32;
+  static size_t mattr = 48 * 1024;
+  if (msmem > mattr) { CD_CUDA(cudaFuncSetAttribute(ctx_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msmem)); mattr = msmem; }
+  ctx_merge_kernel<<<dim3(4, B), 256, msmem, st>>>(ws, nblk, kmax, ksum, ctx);
   CD_LAUNCH_CHECK();
   return 0;
 }

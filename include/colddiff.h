@@ -275,6 +275,9 @@ int cd_add(const float* a, int a_ld, const float* b, int b_ld, float* out, int o
  *   cd_blur_step_down : out = x_t - A_t xhat A_t^T + A_{t-1} xhat A_{t-1}^T    -- DB:451
  * Images are reference-layout NCHW planes.  collapse_last: `discrete` mean-collapse for the
  * last operator index (DB:938-940); quantize: 8-bit truncation (DB:954-958).
+ * Image sizes: S % 4 == 0 and 4 <= S <= 512.  S <= 128 runs one CTA per plane; 128 < S <= 512
+ * one CTA per 32-row strip, and there `out` must not alias `x` / `xhat` (other strips still
+ * read the plane).  Other sizes return an error.
  * ------------------------------------------------------------------------------------------ */
 int cd_blur_apply(const float* x, float* out, const float* ops, const int64_t* t, int t_scalar,
                   int B, int C, int S, int T, int collapse_last, int quantize, void* stream);
