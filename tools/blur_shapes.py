@@ -1,13 +1,19 @@
 """Time the blur degradation kernels and the deblurring model above 128².
 
     python tools/blur_shapes.py [--json FILE]
+    python tools/blur_shapes.py --size 512 [--json FILE]
 
 - cd_blur_apply (per-sample t) and cd_blur_step_down at S = 128, 256, 512, B = 32, C = 3: microseconds per launch, GFLOP/s
   (4 S^3 FLOP per plane and product), and the bytes the launch must move computed from the shapes, with the bound this implies.
   S = 128 is the one-CTA-per-plane kernel; above it the row-strip kernel, which reads X and A_t from L2 once per 32-row strip.
 - One training step of `Unet(64, (1, 2, 4, 8))` at 256² (B = 8, 16 and 32, one micro-batch, Adam + EMA): images/s and the
   peak device memory of the step, each batch size in a process of its own.
-- One reverse step of `sample` (x0_step_down) at 256², B = 16.
+- One reverse step of `sample` (x0_step_down) at the same size and batch.
+- With --size 512: only the training step and the reverse step at 512², B = 1, 2, 4, 8, 10 and 12 (the kernels are skipped).
+  The reverse step runs in the same process as the training step, as in a Trainer that samples while it trains.  A batch
+  size whose training step runs out of device memory is reported as not fitting, and the larger ones are not tried.  Then
+  the largest batch that trains and samples in one process runs once more with gradient_accumulate_every = 2 (twice the
+  images per optimizer step).
 
 Every number is printed with the card name and power limit read in the same run.  A run without a GPU stops."""
 import argparse
@@ -81,48 +87,69 @@ def kernels(res):
         torch.cuda.empty_cache()
 
 
-def model(res, B):
+def model(res, S, B, A=1):
     """one batch size per process: the caching allocator and the engine's shape-keyed buffers of an earlier batch size would
     otherwise still be allocated and count towards this one's peak"""
-    S, T = 256, 200
+    T = 200
     with contextlib.redirect_stdout(io.StringIO()):
         unet = cdm.Unet(dim=64, dim_mults=(1, 2, 4, 8), channels=3).cuda()
         gd = cdm.GaussianDiffusion(unet, image_size=S, device_of_kernel='cuda', channels=3, timesteps=T, loss_type='l1',
                                    kernel_std=0.01, kernel_size=15, blur_routine='Exponential_reflect',
                                    sampling_routine='x0_step_down').cuda()
         tr = cdm.Trainer(gd, None, image_size=S, train_batch_size=B, train_lr=2e-5, train_num_steps=10 ** 9,
-                         gradient_accumulate_every=1, ema_decay=0.995, fp16=False, results_folder=tempfile.mkdtemp(),
+                         gradient_accumulate_every=A, ema_decay=0.995, fp16=False, results_folder=tempfile.mkdtemp(),
                          dataset='synthetic')
     x = torch.rand(B, 3, S, S, device='cuda') * 2 - 1
     for _ in range(3):
-        tr.train_step([x])
+        tr.train_step([x] * A)
     torch.cuda.synchronize()
     resident = torch.cuda.memory_allocated() / 2 ** 30        # weights, gradients, Adam state, EMA copy, engine buffers
     torch.cuda.reset_peak_memory_stats()
-    us = timed(lambda: tr.train_step([x]), 10)
+    us = timed(lambda: tr.train_step([x] * A), 10)
     peak = torch.cuda.max_memory_allocated() / 2 ** 30
-    r = dict(B=B, S=S, step_ms=us / 1e3, images_per_s=B / (us * 1e-6), peak_gib=peak, resident_gib=resident,
+    r = dict(B=B, S=S, accumulate=A, step_ms=us / 1e3, images_per_s=A * B / (us * 1e-6), peak_gib=peak, resident_gib=resident,
              reserved_gib=torch.cuda.max_memory_reserved() / 2 ** 30)
-    res['train'].append(r)
-    print('train step 256^2 B=%2d: %8.2f ms  %7.1f images/s  peak device memory %.2f GiB (%.2f GiB resident between steps, '
-          '%.2f GiB reserved)' % (B, us / 1e3, r['images_per_s'], peak, resident, r['reserved_gib']))
-    if B == 16:
-        ema = tr.ema_model
-        img = gd.opt(x, T)
-        step = torch.full((B,), T - 1, dtype=torch.long, device='cuda')
+    ema = tr.ema_model
+    img = gd.opt(x, T)
+    step = torch.full((B,), T - 1, dtype=torch.long, device='cuda')
 
-        def reverse():
-            with torch.no_grad():
-                ema._reverse_step(img, ema.denoise_fn(img, step), T)
-        us = timed(reverse, 10)
-        res['reverse_step'] = dict(B=B, S=S, ms=us / 1e3)
-        print('reverse step (x0_step_down) 256^2 B=16: %.2f ms' % (us / 1e3))
+    def reverse():
+        with torch.no_grad():
+            ema._reverse_step(img, ema.denoise_fn(img, step), T)
+    try:
+        r['reverse_ms'] = timed(reverse, 10) / 1e3
+        rev = '%.2f ms' % r['reverse_ms']
+    except torch.cuda.OutOfMemoryError:
+        # the EMA model's engine allocates its own forward buffers next to everything the training step keeps
+        r['reverse_ms'], rev = None, 'out of device memory beside the training state'
+    res['train'].append(r)
+    print('train step %d^2 B=%2d x %d: %8.2f ms  %7.1f images/s  peak device memory %.2f GiB (%.2f GiB resident between steps, '
+          '%.2f GiB reserved)  reverse step (x0_step_down) %s' % (S, B, A, us / 1e3, r['images_per_s'], peak, resident,
+                                                                r['reserved_gib'], rev))
+
+
+def measure(res, S, B, A):
+    """one training step size in a fresh process -> False when it ran out of device memory"""
+    with tempfile.NamedTemporaryFile(suffix='.json') as f:
+        p = subprocess.run([sys.executable, os.path.abspath(__file__), '--size', str(S), '--batch', str(B), '--accumulate', str(A),
+                            '--json', f.name], capture_output=True, text=True)
+        sys.stdout.write(p.stdout)
+        if p.returncode != 0:
+            if 'OutOfMemoryError' not in p.stderr and 'out of memory' not in p.stderr:
+                sys.exit(p.stderr)
+            res['does_not_fit'] = dict(S=S, B=B, accumulate=A)
+            print('train step %d^2 B=%2d x %d: out of device memory' % (S, B, A))
+            return False
+        res['train'] += json.load(open(f.name))['train']
+    return True
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--json')
-    ap.add_argument('--batch', type=int, help='measure the 256^2 training step at this batch size only')
+    ap.add_argument('--size', type=int, default=256, choices=(256, 512), help='image side of the training step')
+    ap.add_argument('--batch', type=int, help='measure the training step at this batch size only')
+    ap.add_argument('--accumulate', type=int, default=1, help='gradient_accumulate_every of that step')
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit('blur_shapes: no CUDA device; nothing is measured')
@@ -130,15 +157,18 @@ def main():
     print('card: %s, power limit %s' % (name, pl))
     res = dict(card=name, power_limit=pl, kernels=[], train=[])
     if a.batch:
-        model(res, a.batch)
+        model(res, a.size, a.batch, a.accumulate)
     else:
-        kernels(res)
-        for B in (8, 16, 32):
-            with tempfile.NamedTemporaryFile(suffix='.json') as f:
-                subprocess.check_call([sys.executable, os.path.abspath(__file__), '--batch', str(B), '--json', f.name])
-                sub = json.load(open(f.name))
-            res['train'] += sub['train']
-            res.update({k: v for k, v in sub.items() if k == 'reverse_step'})
+        if a.size == 256:
+            kernels(res)
+        fits = None
+        for B in ((8, 16, 32) if a.size == 256 else (1, 2, 4, 8, 10, 12)):
+            if not measure(res, a.size, B, 1):
+                break
+            if res['train'][-1]['reverse_ms'] is not None:
+                fits = B                    # the largest batch that trains and samples in one process
+        if a.size == 512 and fits:
+            measure(res, a.size, fits, 2)
     if a.json:
         with open(a.json, 'w') as f:
             json.dump(res, f, indent=1)
