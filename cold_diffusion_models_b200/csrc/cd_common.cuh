@@ -24,8 +24,8 @@ void cd_set_error(const char* fmt, ...);
 
 static inline int cd_cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-// SM count of the current device for the grid-size heuristics of the CUDA-core kernels (queried once; 132 = H100 SXM if the
-// query fails, which only changes how work is split)
+// SM count of the current device for the grid sizes and grid-size heuristics of every kernel (queried once; 132 = H100 SXM if
+// the query fails, which only changes how work is split)
 static inline int cd_num_sms() {
   static int n = 0;
   if (n <= 0) {

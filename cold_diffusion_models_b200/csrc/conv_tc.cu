@@ -379,55 +379,81 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constan
 // host side
 // ---------------------------------------------------------------------------------------------
 
-int g_num_sms = 0;
 int g_tf32_map_dtype = 1;   // 1: TFLOAT32 tensor maps; 0: FLOAT32 (diagnostic, cd_conv_tc_set_tf32_maps)
 
-
-template <int BN, int STAGES, bool STG = false, bool F16 = false, int CTAS = 1, bool PAIR = false>
-int launch(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
-  constexpr size_t smem = size_t(STAGES) * (kABytes + BN * 128) + 1024 + 256 + (STG ? sizeof(float) * 2 * 64 * kEpiStageStride : 0);
-  static_assert(smem <= 232448, "dynamic shared memory of one CTA (227 KB)");
-  static_assert(CTAS == 1 || 2 * (smem + 1024) <= 233472, "two CTAs per SM must fit the 228 KB of shared memory");
-  auto kern = conv_tc_kernel<BN, STAGES, STG, F16, CTAS, PAIR>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    CD_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_done = true;
-  }
+// Persistent launch of either kernel: at most CTAS CTAs per SM walk the tiles round-robin (PAIR: clusters of two CTAs over the
+// (M tile pair, co tile) units, one cluster per SM pair)
+template <auto Kernel, size_t kSmem, int CTAS, bool PAIR = false>
+int launch_persistent(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
+  static_assert(kSmem <= 232448, "dynamic shared memory of one CTA (227 KB)");
+  static_assert(CTAS == 1 || 2 * (kSmem + 1024) <= 233472, "two CTAs per SM must fit the 228 KB of shared memory");
+  CD_CUDA(smem_limit_once<Kernel>(kSmem));
   if constexpr (PAIR) {
-    const int units = p.tiles_co * ((p.total_tiles / p.tiles_co + 1) / 2), slots = g_num_sms / 2;
+    const int units = p.tiles_co * ((p.total_tiles / p.tiles_co + 1) / 2), slots = cd_num_sms() / 2;
     cudaLaunchConfig_t cfg = {};
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.gridDim = dim3(2 * (units < slots ? units : slots)); cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem; cfg.stream = st; cfg.attrs = attr; cfg.numAttrs = 1;
-    CD_CUDA(cudaLaunchKernelEx(&cfg, kern, maps[0], maps[1], maps[2], maps[3], p));
+    cfg.dynamicSmemBytes = kSmem; cfg.stream = st; cfg.attrs = attr; cfg.numAttrs = 1;
+    CD_CUDA(cudaLaunchKernelEx(&cfg, Kernel, maps[0], maps[1], maps[2], maps[3], p));
   } else {
-    const int slots = g_num_sms * CTAS;
+    const int slots = cd_num_sms() * CTAS;
     const int grid = p.total_tiles < slots ? p.total_tiles : slots;
-    kern<<<grid, kThreads, smem, st>>>(maps[0], maps[1], maps[2], maps[3], p);
+    Kernel<<<grid, kThreads, kSmem, st>>>(maps[0], maps[1], maps[2], maps[3], p);
   }
   CD_LAUNCH_CHECK();
   return 0;
 }
 
+template <int BN, int STAGES, bool STG = false, bool F16 = false, int CTAS = 1, bool PAIR = false>
+int launch(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
+  constexpr size_t smem = size_t(STAGES) * (kABytes + BN * 128) + 1024 + 256 + (STG ? sizeof(float) * 2 * 64 * kEpiStageStride : 0);
+  return launch_persistent<conv_tc_kernel<BN, STAGES, STG, F16, CTAS, PAIR>, smem, CTAS, PAIR>(maps, p, st);
+}
+
 template <int BN, int ABOXES, int STAGES, int CTAS = 1>
 int launch_rows(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
   constexpr size_t smem = size_t(ABOXES) * kRowsBoxBytes + size_t(STAGES) * BN * 128 + 1024 + 256;
-  static_assert(smem <= 232448, "dynamic shared memory of one CTA (227 KB)");
-  static_assert(CTAS == 1 || 2 * (smem + 1024) <= 233472, "two CTAs per SM must fit the 228 KB of shared memory");
-  auto kern = conv_rows_kernel<BN, ABOXES, STAGES, CTAS>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    CD_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_done = true;
+  return launch_persistent<conv_rows_kernel<BN, ABOXES, STAGES, CTAS>, smem, CTAS>(maps, p, st);
+}
+
+// Operand conditions of both kernels: nsrc, 16-byte aligned operands, source channels in whole chunks of chunk_elems and a tap
+// count the descriptor can hold.  With `report` the first failed condition becomes the library's last error.
+bool operands_ok(const CdConvDesc* d, int chunk_elems, int esz, bool report) {
+#define TC_CHECK(cond, ...) do { if (!(cond)) { if (report) cd_set_error(__VA_ARGS__); return false; } } while (0)
+  TC_CHECK(d->nsrc >= 1 && d->nsrc <= 2, "conv_tc: nsrc must be 1 or 2");
+  TC_CHECK(d->act != CD_ACT_GELU_BWD || (d->aux && (reinterpret_cast<uintptr_t>(d->aux) & 15) == 0 && d->aux_ld % 4 == 0), "conv_tc: GELU_BWD needs an aligned aux");
+  TC_CHECK((reinterpret_cast<uintptr_t>(d->out) & 15) == 0 && d->out_ld % 4 == 0, "conv_tc: out must be 16B aligned");
+  TC_CHECK(!d->resid || ((reinterpret_cast<uintptr_t>(d->resid) & 15) == 0 && d->resid_ld % 4 == 0), "conv_tc: resid alignment");
+  TC_CHECK(!d->out2 || ((reinterpret_cast<uintptr_t>(d->out2) & 15) == 0 && d->out2_ld % 4 == 0), "conv_tc: out2 alignment");
+  TC_CHECK(!d->bias || (reinterpret_cast<uintptr_t>(d->bias) & 15) == 0, "conv_tc: bias alignment");
+  for (int s = 0; s < d->nsrc; ++s) {
+    const CdConvSrc& cs = d->s[s];
+    TC_CHECK(cs.C % chunk_elems == 0 && cs.C > 0, "conv_tc: source channels %d not a multiple of %d", cs.C, chunk_elems);
+    TC_CHECK(cs.ntaps >= 1 && cs.ntaps <= CD_MAX_TAPS, "conv_tc: bad ntaps");
+    TC_CHECK((reinterpret_cast<uintptr_t>(cs.src) & 15) == 0 && (cs.ld * esz) % 16 == 0, "conv_tc: src must be 16B aligned");
+    TC_CHECK((reinterpret_cast<uintptr_t>(cs.w) & 15) == 0, "conv_tc: weights must be 16B aligned");
   }
-  const int slots = g_num_sms * CTAS;
-  const int grid = p.total_tiles < slots ? p.total_tiles : slots;
-  kern<<<grid, kThreads, smem, st>>>(maps[0], maps[1], maps[2], maps[3], p);
-  CD_LAUNCH_CHECK();
-  return 0;
+#undef TC_CHECK
+  return true;
+}
+
+// the TcParams fields both kernels take from the descriptor as they are: grid, strides, taps, output and epilogue operands
+// (a single source fills the second slot with the first)
+TcParams desc_params(const CdConvDesc* d, int chunk_elems) {
+  TcParams p{};
+  p.B = d->B; p.Hg = d->Hg; p.Wg = d->Wg; p.sy = d->sy; p.sx = d->sx; p.Cout = d->Cout; p.nsrc = d->nsrc;
+  for (int s = 0; s < 2; ++s) {
+    const CdConvSrc& cs = d->s[s < d->nsrc ? s : 0];
+    p.ntaps[s] = cs.ntaps; p.kchunks[s] = cs.C / chunk_elems; p.wpb[s] = cs.w_per_batch;
+    for (int t = 0; t < cs.ntaps; ++t) { p.dy[s][t] = (int8_t)cs.dy[t]; p.dx[s][t] = (int8_t)cs.dx[t]; }
+  }
+  p.out = d->out; p.out_ld = d->out_ld; p.Ho = d->Ho; p.Wo = d->Wo;
+  p.oys = d->oys; p.oxs = d->oxs; p.oy0 = d->oy0; p.ox0 = d->ox0;
+  p.bias = d->bias; p.resid = d->resid; p.resid_ld = d->resid_ld; p.act = d->act; p.round_tf32 = d->round_tf32;
+  p.out2 = d->out2; p.out2_ld = d->out2_ld; p.aux = d->aux; p.aux_ld = d->aux_ld;
+  return p;
 }
 
 }  // namespace
@@ -493,17 +519,10 @@ static int conv_fwd_tc_impl(const CdConvDesc* d, cudaStream_t st, bool f16) {
       if (r <= 0) return r;                                   // 1 = not eligible
     }
   }
-  const int chunk_elems = f16 ? 64 : kChunkK;
-  const int esz = f16 ? 2 : 4;
-  EncodeTiledFn enc = get_encode();
-  CD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
-  if (!g_num_sms) {
-    int dev = 0; CD_CUDA(cudaGetDevice(&dev));
-    CD_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
-  }
-  CD_REQUIRE(d->nsrc >= 1 && d->nsrc <= 2, "conv_tc: nsrc must be 1 or 2");
-  TcParams p{};
-  p.B = d->B; p.Hg = d->Hg; p.Wg = d->Wg; p.sy = d->sy; p.sx = d->sx; p.Cout = d->Cout; p.nsrc = d->nsrc;
+  const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : (g_tf32_map_dtype ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
+  const int esz = map_elem_bytes(dt), chunk_elems = 128 / esz;
+  if (!operands_ok(d, chunk_elems, esz, true)) return -1;
+  TcParams p = desc_params(d, chunk_elems);
   // tile geometry: 128 GEMM rows = TW x TH x TN pixels
   if (d->Wg >= 128) {
     CD_REQUIRE(d->Wg % 128 == 0, "conv_tc: Wg >= 128 must be a multiple of 128 (got %d)", d->Wg);
@@ -526,60 +545,30 @@ static int conv_fwd_tc_impl(const CdConvDesc* d, cudaStream_t st, bool f16) {
                       (g_epi_staged == 3 && kiters_host <= kStagedMidKIters));
   bool pair = false;
   const long long mt = static_cast<long long>(p.tiles_x) * p.tiles_y * p.tiles_n;
+  const int sms = cd_num_sms();
   if (BN == 256) {
     // small spatial sizes (16^2, 32^2) give few M tiles: take the narrower N tile only when it saves whole waves
-    double best = tc_cost(mt, d->Cout, 256, g_num_sms);
-    if (tc_cost(mt, d->Cout, 128, g_num_sms) < best) { BN = 128; best = tc_cost(mt, d->Cout, 128, g_num_sms); }
-    if (!f16 && !staged && g_use_2cta && mt >= 2 && (g_use_2cta == 2 || tc_cost(mt, d->Cout, 256, g_num_sms, true) < best)) {
+    double best = tc_cost(mt, d->Cout, 256, sms);
+    if (tc_cost(mt, d->Cout, 128, sms) < best) { BN = 128; best = tc_cost(mt, d->Cout, 128, sms); }
+    if (!f16 && !staged && g_use_2cta && mt >= 2 && (g_use_2cta == 2 || tc_cost(mt, d->Cout, 256, sms, true) < best)) {
       BN = 256; pair = true;
     }
-  } else if (!f16 && !staged && g_use_2cta && (g_2cta_bn & BN) && d->Cout % BN == 0 && (g_use_2cta == 2 || mt >= 2 * g_num_sms)) {
+  } else if (!f16 && !staged && g_use_2cta && (g_2cta_bn & BN) && d->Cout % BN == 0 && (g_use_2cta == 2 || mt >= 2 * sms)) {
     pair = true;                                              // narrow pair tile: only with at least one pair tile per SM pair
   }
   p.tiles_co = cd_cdiv(d->Cout, BN);
   p.total_tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.tiles_co;
-  p.out = d->out; p.out_ld = d->out_ld; p.Ho = d->Ho; p.Wo = d->Wo;
-  p.oys = d->oys; p.oxs = d->oxs; p.oy0 = d->oy0; p.ox0 = d->ox0;
-  p.bias = d->bias; p.resid = d->resid; p.resid_ld = d->resid_ld; p.act = d->act; p.round_tf32 = d->round_tf32;
-  p.out2 = d->out2; p.out2_ld = d->out2_ld; p.aux = d->aux; p.aux_ld = d->aux_ld;
-  CD_REQUIRE(d->act != CD_ACT_GELU_BWD || (d->aux && (reinterpret_cast<uintptr_t>(d->aux) & 15) == 0 && d->aux_ld % 4 == 0), "conv_tc: GELU_BWD needs an aligned aux");
-  CD_REQUIRE((reinterpret_cast<uintptr_t>(d->out) & 15) == 0 && d->out_ld % 4 == 0, "conv_tc: out must be 16B aligned");
-  CD_REQUIRE(!d->resid || ((reinterpret_cast<uintptr_t>(d->resid) & 15) == 0 && d->resid_ld % 4 == 0), "conv_tc: resid alignment");
-  CD_REQUIRE(!d->out2 || ((reinterpret_cast<uintptr_t>(d->out2) & 15) == 0 && d->out2_ld % 4 == 0), "conv_tc: out2 alignment");
-  CD_REQUIRE(!d->bias || (reinterpret_cast<uintptr_t>(d->bias) & 15) == 0, "conv_tc: bias alignment");
 
   CUtensorMap maps[4];
-  const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : (g_tf32_map_dtype ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
   for (int s = 0; s < 2; ++s) {
     const CdConvSrc& cs = d->s[s < d->nsrc ? s : 0];
-    CD_REQUIRE(cs.C % chunk_elems == 0 && cs.C > 0, "conv_tc: source channels %d not a multiple of %d", cs.C, chunk_elems);
-    CD_REQUIRE(cs.ntaps >= 1 && cs.ntaps <= CD_MAX_TAPS, "conv_tc: bad ntaps");
-    CD_REQUIRE((reinterpret_cast<uintptr_t>(cs.src) & 15) == 0 && (cs.ld * esz) % 16 == 0, "conv_tc: src must be 16B aligned");
-    CD_REQUIRE((reinterpret_cast<uintptr_t>(cs.w) & 15) == 0, "conv_tc: weights must be 16B aligned");
     CD_REQUIRE(!cs.w_per_batch || p.TN == 1, "conv_tc: per-batch weights need >=128 pixels per image");
-    p.ntaps[s] = cs.ntaps; p.kchunks[s] = cs.C / chunk_elems; p.wpb[s] = cs.w_per_batch;
-    for (int t = 0; t < cs.ntaps; ++t) { p.dy[s][t] = (int8_t)cs.dy[t]; p.dx[s][t] = (int8_t)cs.dx[t]; }
-    {   // A: NHWC activations, dims {C, W, H, N}
-      cuuint64_t dims[4] = {(cuuint64_t)cs.C, (cuuint64_t)cs.W, (cuuint64_t)cs.H, (cuuint64_t)d->B};
-      cuuint64_t strides[3] = {(cuuint64_t)cs.ld * esz, (cuuint64_t)cs.ld * esz * cs.W, (cuuint64_t)cs.ld * esz * cs.W * cs.H};
-      cuuint32_t box[4] = {(cuuint32_t)chunk_elems, (cuuint32_t)(p.TW * d->sx), (cuuint32_t)(p.TH * d->sy), (cuuint32_t)p.TN};
-      cuuint32_t estr[4] = {1, (cuuint32_t)d->sx, (cuuint32_t)d->sy, 1};
-      CUresult r = enc(&maps[s], dt, 4, const_cast<float*>(cs.src), dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(A%d) failed: %d", s, (int)r);
-    }
-    {   // B: packed weights, dims {Cin, Cout, ntaps * (per-batch ? B : 1)}
-      const int BNl = BN;
-      cuuint64_t dims[3] = {(cuuint64_t)cs.C, (cuuint64_t)d->Cout, (cuuint64_t)cs.ntaps * (cs.w_per_batch ? d->B : 1)};
-      cuuint64_t strides[2] = {(cuuint64_t)cs.C * esz, (cuuint64_t)cs.C * esz * d->Cout};
-      cuuint32_t box[3] = {(cuuint32_t)chunk_elems, (cuuint32_t)(pair ? BNl / 2 : BNl), 1};   // pair: each CTA fetches half
-      cuuint32_t estr[3] = {1, 1, 1};
-      CUresult r = enc(&maps[2 + s], dt, 3, const_cast<float*>(cs.w), dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(B%d) failed: %d", s, (int)r);
-    }
+    // B: per-batch weight sets follow one another along the tap axis; in SM-pair mode each CTA fetches half of the tile
+    if (!encode_nhwc(&maps[s], dt, cs.src, cs.ld, cs.C, cs.W, cs.H, d->B, 1, 1, 0, 0, p.TW * d->sx, p.TH * d->sy, p.TN, d->sx, d->sy,
+                     s ? "A1" : "A0") ||
+        !encode_weights(&maps[2 + s], dt, cs.w, cs.C, d->Cout, cs.ntaps * (cs.w_per_batch ? d->B : 1), pair ? BN / 2 : BN,
+                        s ? "B1" : "B0"))
+      return -1;
   }
   if (f16) {
     if (BN == 256) return launch<256, 4, false, true>(maps, p, st);
@@ -597,7 +586,7 @@ static int conv_fwd_tc_impl(const CdConvDesc* d, cudaStream_t st, bool f16) {
     return launch<64, 8, false, false, 1, true>(maps, p, st);
   }
   // two CTAs per SM only with more than one wave of tiles: a single wave would pair CTAs on some SMs and leave others idle
-  const int ctas2 = p.total_tiles > g_num_sms ? g_ctas2 : 0;
+  const int ctas2 = p.total_tiles > sms ? g_ctas2 : 0;
   if (BN == 256) return launch<256, 4>(maps, p, st);
   if (BN == 128) return (ctas2 & 128) ? launch<128, 3, false, false, 2>(maps, p, st) : launch<128, 6>(maps, p, st);
   return (ctas2 & 64) ? launch<64, 4, false, false, 2>(maps, p, st) : launch<64, 8>(maps, p, st);
@@ -607,27 +596,13 @@ static int conv_fwd_tc_impl(const CdConvDesc* d, cudaStream_t st, bool f16) {
 // whose tap columns hold three taps each on average (dense 3x3; 1x1 and transposed-convolution parity tap lists stay per-tap) --
 // or, with by_shape, when the per-tap kernel is the faster one for this shape (see the measurement above g_use_2cta)
 static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, bool by_shape) {
-  if (d->sy != 1 || d->sx != 1 || d->nsrc < 1 || d->nsrc > 2) return 1;
+  if (d->sy != 1 || d->sx != 1 || !operands_ok(d, kChunkK, 4, false)) return 1;
   for (int s = 0; s < d->nsrc; ++s) {
     const CdConvSrc& cs = d->s[s];
-    if (cs.w_per_batch || cs.C % kChunkK != 0 || cs.C <= 0 || cs.ntaps < 1 || cs.ntaps > CD_MAX_TAPS) return 1;
-    if (cs.W != d->Wg || cs.H != d->Hg) return 1;
+    if (cs.w_per_batch || cs.W != d->Wg || cs.H != d->Hg) return 1;
     for (int t = 0; t < cs.ntaps; ++t) if (cs.dy[t] < -1 || cs.dy[t] > 1 || cs.dx[t] < -1 || cs.dx[t] > 1) return 1;
-    if ((reinterpret_cast<uintptr_t>(cs.src) & 15) || (cs.ld * 4) % 16 || (reinterpret_cast<uintptr_t>(cs.w) & 15)) return 1;
   }
-  if ((reinterpret_cast<uintptr_t>(d->out) & 15) || d->out_ld % 4) return 1;
-  if (d->resid && ((reinterpret_cast<uintptr_t>(d->resid) & 15) || d->resid_ld % 4)) return 1;
-  if (d->out2 && ((reinterpret_cast<uintptr_t>(d->out2) & 15) || d->out2_ld % 4)) return 1;
-  if (d->bias && (reinterpret_cast<uintptr_t>(d->bias) & 15)) return 1;
-  if (d->act == CD_ACT_GELU_BWD && (!d->aux || (reinterpret_cast<uintptr_t>(d->aux) & 15) || d->aux_ld % 4)) return 1;
-  EncodeTiledFn enc = get_encode();
-  CD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
-  if (!g_num_sms) {
-    int dev = 0; CD_CUDA(cudaGetDevice(&dev));
-    CD_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
-  }
-  TcParams p{};
-  p.B = d->B; p.Hg = d->Hg; p.Wg = d->Wg; p.sy = 1; p.sx = 1; p.Cout = d->Cout; p.nsrc = d->nsrc;
+  TcParams p = desc_params(d, kChunkK);
   p.TW = kRowsTW; p.TH = kRowsTH; p.TN = 1;
   p.tiles_x = cd_cdiv(d->Wg, kRowsTW); p.tiles_y = cd_cdiv(d->Hg, kRowsTH); p.tiles_n = d->B;
   // N tiles of at most 128 columns: two CTAs per SM fit (three boxes and three / six weight tiles each), so one CTA's epilogue
@@ -638,17 +613,12 @@ static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, bool by_shape) {
   p.total_tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.tiles_co;
   // by shape: when the tiles fill more than one wave (a single wave, e.g. the 16^2 layers with Cout = 256, runs faster on the
   // per-tap kernel)
-  if (by_shape && p.total_tiles <= g_num_sms) return 1;
-  p.out = d->out; p.out_ld = d->out_ld; p.Ho = d->Ho; p.Wo = d->Wo;
-  p.oys = d->oys; p.oxs = d->oxs; p.oy0 = d->oy0; p.ox0 = d->ox0;
-  p.bias = d->bias; p.resid = d->resid; p.resid_ld = d->resid_ld; p.act = d->act; p.round_tf32 = d->round_tf32;
-  p.out2 = d->out2; p.out2_ld = d->out2_ld; p.aux = d->aux; p.aux_ld = d->aux_ld;
+  const int sms = cd_num_sms();
+  if (by_shape && p.total_tiles <= sms) return 1;
   const CUtensorMapDataType dt = g_tf32_map_dtype ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUtensorMap maps[4];
   for (int s = 0; s < 2; ++s) {
     const CdConvSrc& cs = d->s[s < d->nsrc ? s : 0];
-    p.ntaps[s] = cs.ntaps; p.kchunks[s] = cs.C / kChunkK; p.wpb[s] = 0;
-    p.nbox[s] = 0;
     int i = 0;
     for (int dx = -1; dx <= 1; ++dx) {                       // taps grouped by column: one box per column present
       const int i0 = i;
@@ -657,30 +627,14 @@ static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, bool by_shape) {
       if (i > i0) { p.boxdx[s][p.nbox[s]] = (int8_t)dx; p.boxend[s][p.nbox[s]] = (int8_t)i; ++p.nbox[s]; }
     }
     if (s == 0 && cs.ntaps < 3 * p.nbox[0]) return 1;
-    for (int t = 0; t < cs.ntaps; ++t) { p.dy[s][t] = (int8_t)cs.dy[t]; p.dx[s][t] = (int8_t)cs.dx[t]; }
-    {   // A: NHWC activations, one box {32 ch, 16, 8 + 2, 1} per chunk and tap column
-      cuuint64_t dims[4] = {(cuuint64_t)cs.C, (cuuint64_t)cs.W, (cuuint64_t)cs.H, (cuuint64_t)d->B};
-      cuuint64_t strides[3] = {(cuuint64_t)cs.ld * 4, (cuuint64_t)cs.ld * 4 * cs.W, (cuuint64_t)cs.ld * 4 * cs.W * cs.H};
-      cuuint32_t box[4] = {(cuuint32_t)kChunkK, (cuuint32_t)kRowsTW, (cuuint32_t)(kRowsTH + 2), 1};
-      cuuint32_t estr[4] = {1, 1, 1, 1};
-      CUresult r = enc(&maps[s], dt, 4, const_cast<float*>(cs.src), dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(rows A%d) failed: %d", s, (int)r);
-    }
-    {   // B: packed weights [tap][Cout][Cin]
-      cuuint64_t dims[3] = {(cuuint64_t)cs.C, (cuuint64_t)d->Cout, (cuuint64_t)cs.ntaps};
-      cuuint64_t strides[2] = {(cuuint64_t)cs.C * 4, (cuuint64_t)cs.C * 4 * d->Cout};
-      cuuint32_t box[3] = {(cuuint32_t)kChunkK, (cuuint32_t)BN, 1};
-      cuuint32_t estr[3] = {1, 1, 1};
-      CUresult r = enc(&maps[2 + s], dt, 3, const_cast<float*>(cs.w), dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(rows B%d) failed: %d", s, (int)r);
-    }
+    // A: one box {32 ch, 16, 8 + 2, 1} per chunk and tap column
+    if (!encode_nhwc(&maps[s], dt, cs.src, cs.ld, cs.C, cs.W, cs.H, d->B, 1, 1, 0, 0, kRowsTW, kRowsTH + 2, 1, 1, 1,
+                     s ? "rows A1" : "rows A0") ||
+        !encode_weights(&maps[2 + s], dt, cs.w, cs.C, d->Cout, cs.ntaps, BN, s ? "rows B1" : "rows B0"))
+      return -1;
   }
   // one CTA per SM: six boxes (120 KB) and 64 KB of weight tiles; two CTAs per SM: three boxes and 48 KB of weight tiles each
-  const int ctas2 = p.total_tiles > g_num_sms ? g_ctas2 : 0;
+  const int ctas2 = p.total_tiles > sms ? g_ctas2 : 0;
   if (BN == 128) return (ctas2 & 128) ? launch_rows<128, 3, 3, 2>(maps, p, st) : launch_rows<128, 6, 4>(maps, p, st);
   return (ctas2 & 64) ? launch_rows<64, 3, 6, 2>(maps, p, st) : launch_rows<64, 6, 8>(maps, p, st);
 }

@@ -191,18 +191,15 @@ dwconv7_wgrad_tma_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_
 }
 
 int g_dw_tma = 1;
-int g_sms_dw = 0;
 
 // plain fp32 tiles, no swizzle, zero fill outside the image
 bool make_map(CUtensorMap* m, const float* p, int ld, int B, int H, int W, int C, int bx, int by) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return false;
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)ld * 4, (cuuint64_t)ld * 4 * W, (cuuint64_t)ld * 4 * W * H};
-  cuuint32_t box[4] = {32, (cuuint32_t)bx, (cuuint32_t)by, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(p), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+  const cuuint64_t strides[3] = {(cuuint64_t)ld * 4, (cuuint64_t)ld * 4 * W, (cuuint64_t)ld * 4 * W * H};
+  const cuuint32_t box[4] = {32, (cuuint32_t)bx, (cuuint32_t)by, 1};
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  return encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, p, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE,
+                      CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "dwconv7");
 }
 
 }  // namespace
@@ -218,19 +215,11 @@ int cd_dwconv7_fwd_tma(const float* x, int x_ld, int B, int H, int W, int C, con
   CUtensorMap mapX;
   if (!make_map(&mapX, x, x_ld, B, H, W, C, TX + 6, kTY + 6)) return 1;
   const size_t smem = sizeof(float) * 2 * 32 * size_t(kTY + 6) * (TX + 6) + 128;
-  static bool attr = false;
-  if (!attr) {
-    CD_CUDA(cudaFuncSetAttribute(dwconv7_tma_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * 2 * 32 * (kTY + 6) * 38 + 128)));
-    CD_CUDA(cudaFuncSetAttribute(dwconv7_tma_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * 2 * 32 * (kTY + 6) * 22 + 128)));
-    attr = true;
-  }
-  if (!g_sms_dw) { int dev = 0; CD_CUDA(cudaGetDevice(&dev)); CD_CUDA(cudaDeviceGetAttribute(&g_sms_dw, cudaDevAttrMultiProcessorCount, dev)); }
+  CD_CUDA(TX == 32 ? smem_limit_once<dwconv7_tma_kernel<32>>(smem) : smem_limit_once<dwconv7_tma_kernel<16>>(smem));
   const long long total = static_cast<long long>(C / 32) * B * (H / kTY) * (W / TX);
-  const int grid = total < g_sms_dw ? static_cast<int>(total) : g_sms_dw;
-  if (TX == 32)
-    dwconv7_tma_kernel<32><<<grid, 32 * kTY, smem, st>>>(mapX, B, H, W, C, w_dw, b_dw, cond, cond_ld, out, out_ld, flip, addend, addend_ld);
-  else
-    dwconv7_tma_kernel<16><<<grid, 32 * kTY, smem, st>>>(mapX, B, H, W, C, w_dw, b_dw, cond, cond_ld, out, out_ld, flip, addend, addend_ld);
+  const int grid = total < cd_num_sms() ? static_cast<int>(total) : cd_num_sms();
+  auto kern = TX == 32 ? dwconv7_tma_kernel<32> : dwconv7_tma_kernel<16>;
+  kern<<<grid, 32 * kTY, smem, st>>>(mapX, B, H, W, C, w_dw, b_dw, cond, cond_ld, out, out_ld, flip, addend, addend_ld);
   CD_LAUNCH_CHECK();
   return 0;
 }
@@ -241,11 +230,9 @@ int cd_dwconv7_wgrad_tma(const float* dh, int dh_ld, const float* x, int x_ld, i
   CUtensorMap mapX, mapD;
   if (!make_map(&mapX, x, x_ld, B, H, W, C, kWTX + 6, kTY + 6) || !make_map(&mapD, dh, dh_ld, B, H, W, C, kWTX, kTY)) return 1;
   const size_t smem = sizeof(float) * 2 * 32 * (size_t(kTY + 6) * (kWTX + 6) + size_t(kTY) * kWTX) + 128;
-  static bool attr = false;
-  if (!attr) { CD_CUDA(cudaFuncSetAttribute(dwconv7_wgrad_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
-  if (!g_sms_dw) { int dev = 0; CD_CUDA(cudaGetDevice(&dev)); CD_CUDA(cudaDeviceGetAttribute(&g_sms_dw, cudaDevAttrMultiProcessorCount, dev)); }
+  CD_CUDA(smem_limit_once<dwconv7_wgrad_tma_kernel>(smem));
   const long long total = static_cast<long long>(C / 32) * B * (H / kTY) * (W / kWTX);
-  const int grid = total < g_sms_dw ? static_cast<int>(total) : g_sms_dw;
+  const int grid = total < cd_num_sms() ? static_cast<int>(total) : cd_num_sms();
   dwconv7_wgrad_tma_kernel<<<grid, 32 * kTY, smem, st>>>(mapX, mapD, B, H, W, C, dw);
   CD_LAUNCH_CHECK();
   return 0;

@@ -772,10 +772,8 @@ int cd_dwconv7_wgrad_pipe(const float* dh, int dh_ld, const float* x, int x_ld, 
   const size_t smem = sizeof(float) * 2 * 32 * (size_t(kDwPTY + 6) * (kDwWTX + 6) + size_t(kDwPTY) * kDwWTX);
   static bool attr = false;
   if (!attr) { CD_CUDA(cudaFuncSetAttribute(dwconv7_wgrad_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
-  static int sms = 0;
-  if (!sms) { int dev = 0; CD_CUDA(cudaGetDevice(&dev)); CD_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)); }
   const long long total = static_cast<long long>(C / 32) * B * (H / kDwPTY) * (W / kDwWTX);
-  const int grid = total < sms ? static_cast<int>(total) : sms;
+  const int grid = total < cd_num_sms() ? static_cast<int>(total) : cd_num_sms();
   dwconv7_wgrad_pipe_kernel<<<grid, 32 * kDwPTY, smem, st>>>(dh, dh_ld, x, x_ld, B, H, W, C, dw);
   CD_LAUNCH_CHECK();
   return 0;
@@ -798,10 +796,8 @@ extern "C" int cd_dwconv7_fwd(const float* x, int x_ld, int B, int H, int W, int
       CD_CUDA(cudaFuncSetAttribute(dwconv7_pipe_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(float) * 2 * 32 * (kDwPTY + 6) * 22)));
       attr_p = true;
     }
-    static int sms = 0;
-    if (!sms) { int dev = 0; CD_CUDA(cudaGetDevice(&dev)); CD_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)); }
     const long long total = static_cast<long long>(C / 32) * B * (H / kDwPTY) * (W / TXp);
-    const int grid = total < sms ? static_cast<int>(total) : sms;
+    const int grid = total < cd_num_sms() ? static_cast<int>(total) : cd_num_sms();
     if (TXp == 32)
       dwconv7_pipe_kernel<32><<<grid, 32 * kDwPTY, smem, static_cast<cudaStream_t>(stream)>>>(x, x_ld, B, H, W, C, w_dw, b_dw, cond, cond_ld,
                                                                                             out, out_ld, flip, addend, addend_ld);
@@ -861,12 +857,10 @@ extern "C" int cd_linattn_context(const float* qkv, int ld, int B, int n, float*
   const int variant = cd_linattn_staged_enabled(nullptr, nullptr) ? 1 : 0;     // the PRELOAD kernel holds 32 more registers
   static int slots_v[2] = {0, 0};
   if (!slots_v[variant]) {
-    int dev = 0, sms = 0, occ = 0;
-    CD_CUDA(cudaGetDevice(&dev));
-    CD_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int occ = 0;
     if (variant) CD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, context_kernel<true>, 256, 0));
     else CD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, context_kernel<false>, 256, 0));
-    slots_v[variant] = sms * (occ > 0 ? occ : 1);
+    slots_v[variant] = cd_num_sms() * (occ > 0 ? occ : 1);
   }
   const int slots = slots_v[variant];
   int per_img = slots / (B > 0 ? B : 1); if (per_img < 1) per_img = 1;

@@ -156,14 +156,12 @@ int cd_linattn_bwd_kv_mma(const float* qkv, int ld, int B, int n, const float* k
                           const float* rowdot, float* dqkv, int dld, cudaStream_t st) {
   if (!g_bwd_mma || ld % 4 != 0 || dld % 2 != 0 || (reinterpret_cast<uintptr_t>(qkv) & 15) != 0 || (reinterpret_cast<uintptr_t>(dqkv) & 7) != 0)
     return 1;
-  static int sms = 0;
-  if (!sms) { int dev = 0; CD_CUDA(cudaGetDevice(&dev)); CD_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)); }
   const size_t smem = sizeof(float) * (2 * 4 * 32 * kLc + 3 * 128 + 2 * 2 * kP * kLd);
   static bool attr = false;
   if (!attr) { CD_CUDA(cudaFuncSetAttribute(attn_bwd_kv_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
   // spans of ppb pixels (a multiple of 32): about one wave of resident blocks (2 per SM) over the batch; the 42 KB of per-image
   // operands are staged once per block, so spans are not made shorter than 4 tiles
-  int per_img = 2 * sms / B; if (per_img < 1) per_img = 1;
+  int per_img = 2 * cd_num_sms() / B; if (per_img < 1) per_img = 1;
   int ppb = cd_cdiv(cd_cdiv(n, per_img), kP) * kP;
   if (ppb < 4 * kP) ppb = 4 * kP;
   attn_bwd_kv_mma_kernel<<<dim3(cd_cdiv(n, ppb), B), 256, smem, st>>>(qkv, ld, n, ppb, kmax, ksum, dctxn, rowdot, dqkv, dld);

@@ -1,6 +1,6 @@
-// Device / host helpers shared by the tensor-core translation units (conv_tc.cu, wgrad_tc.cu): mbarrier and TMA wrappers,
-// the K-major SWIZZLE_128B wgmma shared-memory descriptor, wgmma issue / fence / commit / wait, and the cuTensorMapEncodeTiled
-// entry point.  Everything lives in an unnamed namespace: each translation unit gets its own copy.
+// Device / host helpers shared by the TMA translation units (conv_tc.cu, wgrad_tc.cu, dwconv_tma.cu): mbarrier and TMA wrappers,
+// the K-major SWIZZLE_128B wgmma shared-memory descriptor, wgmma issue / fence / commit / wait, and on the host the tensor-map
+// encoders and the dynamic shared-memory opt-in.  Everything lives in an unnamed namespace: each translation unit gets its own copy.
 #pragma once
 #include "cd_common.cuh"
 
@@ -177,6 +177,58 @@ EncodeTiledFn get_encode() {
       fn = reinterpret_cast<EncodeTiledFn>(p);
   }
   return fn;
+}
+
+// cuTensorMapEncodeTiled without interleave or out-of-bounds NaN fill (the border reads as zeros); on failure the library's last
+// error names the map (`what`) and false is returned
+bool encode_tiled(CUtensorMap* m, CUtensorMapDataType dt, cuuint32_t rank, const void* base, const cuuint64_t* dims,
+                  const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapSwizzle swizzle,
+                  CUtensorMapL2promotion l2, const char* what) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) { cd_set_error("cuTensorMapEncodeTiled entry point unavailable"); return false; }
+  const CUresult r = enc(m, dt, rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                         l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) cd_set_error("cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r);
+  return r == CUDA_SUCCESS;
+}
+
+int map_elem_bytes(CUtensorMapDataType dt) { return dt == CU_TENSOR_MAP_DATA_TYPE_FLOAT16 ? 2 : 4; }
+
+// NHWC activations (W x H pixels per image, pixels ld elements apart) as the 4-D map {C, W / gx, H / gy, B} whose pixel (x, y) is
+// image pixel (ex + gx x, ey + gy y): gx / gy multiply the byte strides.  A box is one 128-byte swizzle row of channels by bw x bh
+// map pixels of bn images, of which it takes every sx-th pixel and sy-th row (element strides).  SWIZZLE_128B, L2 promotion 128 B.
+bool encode_nhwc(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int ld, int C, int W, int H, int B, int gx, int gy,
+                 int ex, int ey, int bw, int bh, int bn, int sx, int sy, const char* what) {
+  const int esz = map_elem_bytes(dt);
+  const cuuint64_t pix = (cuuint64_t)ld * esz;
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)(W / gx), (cuuint64_t)(H / gy), (cuuint64_t)B};
+  const cuuint64_t strides[3] = {pix * gx, pix * W * gy, pix * W * H};
+  const cuuint32_t box[4] = {(cuuint32_t)(128 / esz), (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
+  const cuuint32_t estr[4] = {1, (cuuint32_t)sx, (cuuint32_t)sy, 1};
+  return encode_tiled(m, dt, 4, static_cast<const uint8_t*>(base) + (static_cast<long long>(ey) * W + ex) * pix, dims, strides, box,
+                      estr, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, what);
+}
+
+// packed weights [taps][Cout][Cin] as the 3-D map {Cin, Cout, taps}; a box is one 128-byte swizzle row of Cin by bco output
+// channels of one tap.  SWIZZLE_128B, L2 promotion 256 B.
+bool encode_weights(CUtensorMap* m, CUtensorMapDataType dt, const void* w, int Cin, int Cout, int taps, int bco, const char* what) {
+  const int esz = map_elem_bytes(dt);
+  const cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)Cout, (cuuint64_t)taps};
+  const cuuint64_t strides[2] = {(cuuint64_t)Cin * esz, (cuuint64_t)Cin * esz * Cout};
+  const cuuint32_t box[3] = {(cuuint32_t)(128 / esz), (cuuint32_t)bco, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  return encode_tiled(m, dt, 3, w, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
+}
+
+// Lets Kernel use `bytes` of dynamic shared memory.  The attribute is set on the first successful call only, so a kernel whose
+// launches differ in size passes the largest size any launch can request.
+template <auto Kernel>
+cudaError_t smem_limit_once(size_t bytes) {
+  static bool done = false;
+  if (done) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+  done = e == cudaSuccess;
+  return e;
 }
 
 bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }

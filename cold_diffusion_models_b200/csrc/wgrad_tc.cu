@@ -475,18 +475,18 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap mapDY, const __grid_const
 }
 
 int g_wg_mode = 1;      // 0: one X tile per tap (mma.sync); 8: mma.sync halo kernel; otherwise (default) the wgmma kernel where eligible
-int g_sms = 0;
+
+// largest dynamic shared memory a launch of either kernel requests: at most 224 KB of stages + 1024-byte alignment slack +
+// barrier block
+constexpr int kMaxSmem = 224 * 1024 + 1024 + 256;
 
 template <int BN, int NT>
 int launch_wg(bool bias, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& mapDY, const CUtensorMap& mapX,
               const WgParams& p, int stages, int a_bytes, int b_bytes, int b_tx) {
-  if (bias) {
-    CD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<BN, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    wgrad_tc_kernel<BN, NT, true><<<grid, kThreads, smem, st>>>(mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
-  } else {
-    CD_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<BN, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    wgrad_tc_kernel<BN, NT, false><<<grid, kThreads, smem, st>>>(mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
-  }
+  constexpr auto with_bias = wgrad_tc_kernel<BN, NT, true>, without = wgrad_tc_kernel<BN, NT, false>;
+  CD_CUDA(bias ? smem_limit_once<with_bias>(kMaxSmem) : smem_limit_once<without>(kMaxSmem));
+  auto kern = bias ? with_bias : without;
+  kern<<<grid, kThreads, smem, st>>>(mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx);
   CD_LAUNCH_CHECK();
   return 0;
 }
@@ -506,7 +506,8 @@ static int g_split_policy = 3;
 static int g_split_over_clk = 12000;     // fixed cost per CTA in SM clocks (prologue + first-load latency + red.add epilogue)
 extern "C" int cd_wgrad_tc_set_split(int policy, int over_clk) { g_split_policy = policy; if (over_clk > 0) g_split_over_clk = over_clk; return 0; }
 
-static int choose_splits(int tg, int total_chunks, int max_splits, int sms, double chunk_clk) {
+static int choose_splits(int tg, int total_chunks, int max_splits, double chunk_clk) {
+  const int sms = cd_num_sms();
   if (max_splits < 1) max_splits = 1;
   int s;
   if (g_split_policy == 0) s = cd_cdiv(2 * sms, tg);
@@ -526,35 +527,15 @@ static int choose_splits(int tg, int total_chunks, int max_splits, int sms, doub
   return s;
 }
 
-constexpr int kWmSmem = 224 * 1024 + 1024 + 256;     // stages + 1024-byte alignment slack + barrier block
-
 template <int BN, int NT, int CW, bool HALO>
 static int launch_wm(dim3 grid, cudaStream_t st, const CUtensorMap& mapDY, const CUtensorMap& mapX, const WgParams& p) {
   constexpr int kStage = WmStage<BN, CW, HALO>::kBytes;
   int stages = (224 * 1024) / kStage; if (stages > 5) stages = 5;     // six barriers per stage in the 256-byte barrier block
   const size_t smem = size_t(stages) * kStage + 1024 + 256;
-  auto kern = wgrad_wgmma_kernel<BN, NT, CW, HALO>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    CD_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kWmSmem));
-    attr_done = true;
-  }
+  constexpr auto kern = wgrad_wgmma_kernel<BN, NT, CW, HALO>;
+  CD_CUDA(smem_limit_once<kern>(kMaxSmem));
   kern<<<grid, kWmThreads, smem, st>>>(mapDY, mapX, p, stages);
   CD_LAUNCH_CHECK();
-  return 0;
-}
-
-// NHWC tensor map {C, W, H, B} over the pixels (ey + sy i, ex + sx j) of a W0 x H0 image: dims W x H, box {32, bw, bh, 1}
-static int encode_nhwc(EncodeTiledFn enc, CUtensorMap* m, const float* base, int ld, int C, int W0, int H0, int B, int sy, int sx,
-                        int ey, int ex, int W, int H, int bw, int bh, const char* what) {
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)ld * 4 * sx, (cuuint64_t)ld * 4 * W0 * sy, (cuuint64_t)ld * 4 * W0 * H0};
-  cuuint32_t box[4] = {32, (cuuint32_t)bw, (cuuint32_t)bh, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  float* p = const_cast<float*>(base) + (static_cast<long long>(ey) * W0 + ex) * ld;
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r);
   return 0;
 }
 
@@ -606,7 +587,7 @@ static int wm_plan(const CdConvDesc* d, const WmClass& k, int BN, int CW, WgPara
 // [-1, 1]^2 (3x3, 1x1, the four taps of a transposed-convolution parity class, whose dY is read at every second pixel) and the
 // 4x4 stride-2 downsample, split into its four input-parity classes of four stride-1 taps each (one launch per class, X read at
 // every second pixel).  Cin % 64 == 0 or Cin == 32 (image edge), Cout % 64 == 0, per-batch weights allowed.
-static int wgrad_wgmma(const CdConvDesc* d, const float* dout, int dout_ld, float* dw, EncodeTiledFn enc, cudaStream_t st) {
+static int wgrad_wgmma(const CdConvDesc* d, const float* dout, int dout_ld, float* dw, cudaStream_t st) {
   const CdConvSrc& c = d->s[0];
   if ((c.C % 64 != 0 && c.C != 32) || d->Cout % 64 != 0 || c.ntaps < 1) return 1;
   const bool dense_out = d->oys == 1 && d->oxs == 1 && d->oy0 == 0 && d->ox0 == 0 && d->Ho == d->Hg && d->Wo == d->Wg;
@@ -639,7 +620,9 @@ static int wgrad_wgmma(const CdConvDesc* d, const float* dout, int dout_ld, floa
     if (wm_plan(d, cls[i], BN, CW, ps[i], halo[i])) return 1;
   }
   CUtensorMap mapDY;
-  if (encode_nhwc(enc, &mapDY, dout, dout_ld, d->Cout, d->Wo, d->Ho, d->B, d->oys, d->oxs, d->oy0, d->ox0, d->Wg, d->Hg, CW, R, "wgmma dY")) return -1;
+  if (!encode_nhwc(&mapDY, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dout, dout_ld, d->Cout, d->Wo, d->Ho, d->B, d->oxs, d->oys, d->ox0, d->oy0,
+                   CW, R, 1, 1, 1, "wgmma dY"))
+    return -1;
   for (int i = 0; i < ncls; ++i) {
     WgParams& p = ps[i];
     p.B = d->B; p.Hg = d->Hg; p.Wg = d->Wg; p.Cout = d->Cout; p.Cin = c.C;
@@ -654,19 +637,21 @@ static int wgrad_wgmma(const CdConvDesc* d, const float* dout, int dout_ld, floa
     if (c.w_per_batch) {
       p.per_batch = 1;
       p.chunks_per_img = p.chunks_x * p.chunks_y;
-      const int spi = choose_splits(tiles * p.ngroups * d->B, p.chunks_per_img, p.chunks_per_img, g_sms, chunk_clk);
+      const int spi = choose_splits(tiles * p.ngroups * d->B, p.chunks_per_img, p.chunks_per_img, chunk_clk);
       p.chunks_per_split = cd_cdiv(p.chunks_per_img, spi);
       p.splits_per_img = cd_cdiv(p.chunks_per_img, p.chunks_per_split);
       p.splits = p.splits_per_img * d->B;
       p.dw_batch_stride = static_cast<long long>(c.ntaps) * d->Cout * c.C;
     } else {
-      const int splits = choose_splits(tiles * p.ngroups, p.total_chunks, cd_cdiv(p.total_chunks, 8), g_sms, chunk_clk);
+      const int splits = choose_splits(tiles * p.ngroups, p.total_chunks, cd_cdiv(p.total_chunks, 8), chunk_clk);
       p.chunks_per_split = cd_cdiv(p.total_chunks, splits);
       p.splits = cd_cdiv(p.total_chunks, p.chunks_per_split);
     }
     CUtensorMap mapX;
     const int bw = halo[i] ? CW + 8 : CW, bh = halo[i] ? R + 2 : R;
-    if (encode_nhwc(enc, &mapX, c.src, c.ld, c.C, c.W, c.H, d->B, d->sy, d->sx, cls[i].ey, cls[i].ex, d->Wg, d->Hg, bw, bh, "wgmma X")) return -1;
+    if (!encode_nhwc(&mapX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, c.src, c.ld, c.C, c.W, c.H, d->B, d->sx, d->sy, cls[i].ex, cls[i].ey, bw, bh,
+                     1, 1, 1, "wgmma X"))
+      return -1;
     const dim3 grid(tiles, p.splits, p.ngroups);
 #define WM_LAUNCH(bn, nt, cw) (halo[i] ? launch_wm<bn, nt, cw, true>(grid, st, mapDY, mapX, p) \
                                        : launch_wm<bn, nt, cw, false>(grid, st, mapDY, mapX, p))
@@ -686,12 +671,9 @@ int cd_conv_wgrad_tc(const CdConvDesc* d, const float* dout, int dout_ld, float*
   if (c.C % 32 != 0 || d->Cout % 32 != 0 || c.ld % 4 != 0 || dout_ld % 4 != 0) return 1;
   if (!is_pow2(d->Wg) || d->Wg < 8 || !is_pow2(d->Hg)) return 1;
   if ((reinterpret_cast<uintptr_t>(c.src) & 15) || (reinterpret_cast<uintptr_t>(dout) & 15) || (reinterpret_cast<uintptr_t>(dw) & 15)) return 1;
-  EncodeTiledFn enc = get_encode();
-  CD_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
-  if (!g_sms) { int dev = 0; CD_CUDA(cudaGetDevice(&dev)); CD_CUDA(cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev)); }
   // wgmma kernel wherever eligible, unless a mma.sync kernel is forced (mode 0 / 8) or the bias gradient is to be fused
   if (g_wg_mode != 0 && g_wg_mode != 8 && !(g_wg_bias_fusion && db != nullptr)) {
-    const int r = wgrad_wgmma(d, dout, dout_ld, dw, enc, st);
+    const int r = wgrad_wgmma(d, dout, dout_ld, dw, st);
     if (r <= 0) return r;
   }
 
@@ -745,10 +727,10 @@ int cd_conv_wgrad_tc(const CdConvDesc* d, const float* dout, int dout_ld, float*
   int splits;
   if (c.w_per_batch) {
     const int cpi = p.chunks_x * p.chunks_y;
-    const int spi0 = choose_splits(tiles * p.ngroups * d->B, cpi, cpi, g_sms, chunk_clk);
+    const int spi0 = choose_splits(tiles * p.ngroups * d->B, cpi, cpi, chunk_clk);
     splits = spi0 * d->B;
   } else {
-    splits = choose_splits(tiles * p.ngroups, p.total_chunks, cd_cdiv(p.total_chunks, 8), g_sms, chunk_clk);
+    splits = choose_splits(tiles * p.ngroups, p.total_chunks, cd_cdiv(p.total_chunks, 8), chunk_clk);
   }
   p.chunks_per_split = cd_cdiv(p.total_chunks, splits);
   p.splits = cd_cdiv(p.total_chunks, p.chunks_per_split);
@@ -776,24 +758,11 @@ int cd_conv_wgrad_tc(const CdConvDesc* d, const float* dout, int dout_ld, float*
 
   CUtensorMap mapDY, mapX;
   const CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;   // operands are rounded to TF32 (RN) as they are read
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)d->Cout, (cuuint64_t)d->Wo, (cuuint64_t)d->Ho, (cuuint64_t)d->B};
-    cuuint64_t strides[3] = {(cuuint64_t)dout_ld * 4, (cuuint64_t)dout_ld * 4 * d->Wo, (cuuint64_t)dout_ld * 4 * d->Wo * d->Ho};
-    cuuint32_t box[4] = {32, (cuuint32_t)(p.CW * d->oxs), (cuuint32_t)(p.R * d->oys), 1};
-    cuuint32_t estr[4] = {1, (cuuint32_t)d->oxs, (cuuint32_t)d->oys, 1};
-    CUresult r = enc(&mapDY, dt, 4, const_cast<float*>(dout), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(dY) failed: %d", (int)r);
-  }
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)c.C, (cuuint64_t)c.W, (cuuint64_t)c.H, (cuuint64_t)d->B};
-    cuuint64_t strides[3] = {(cuuint64_t)c.ld * 4, (cuuint64_t)c.ld * 4 * c.W, (cuuint64_t)c.ld * 4 * c.W * c.H};
-    cuuint32_t box[4] = {32, (cuuint32_t)((p.CW + p.halo) * d->sx), (cuuint32_t)(p.R * d->sy), 1};
-    cuuint32_t estr[4] = {1, (cuuint32_t)d->sx, (cuuint32_t)d->sy, 1};
-    CUresult r = enc(&mapX, dt, 4, const_cast<float*>(c.src), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CD_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(X) failed: %d", (int)r);
-  }
+  // boxes of the strided pixel grids, read with element strides
+  if (!encode_nhwc(&mapDY, dt, dout, dout_ld, d->Cout, d->Wo, d->Ho, d->B, 1, 1, 0, 0, p.CW * d->oxs, p.R * d->oys, 1, d->oxs, d->oys,
+                   "dY") ||
+      !encode_nhwc(&mapX, dt, c.src, c.ld, c.C, c.W, c.H, d->B, 1, 1, 0, 0, (p.CW + p.halo) * d->sx, p.R * d->sy, 1, d->sx, d->sy, "X"))
+    return -1;
   dim3 grid(tiles, p.splits, p.ngroups);
   int rc;
   if (BN == 128) rc = max_taps == 1 ? launch_wg<128, 1>(fuse_bias, grid, smem, st, mapDY, mapX, p, stages, a_bytes, b_bytes, b_tx)
