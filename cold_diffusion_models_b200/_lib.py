@@ -65,12 +65,6 @@ if os.environ.get('COLDDIFF_2CTA_BN') in ('0', '64', '128', '192'):   # N tiles 
     lib.cd_conv_tc_set_2cta_bn(int(os.environ['COLDDIFF_2CTA_BN']))
 if os.environ.get('COLDDIFF_CONV_STAGED_EPILOGUE') in ('0', '1', '2', '3'):   # line-coalesced conv epilogue (csrc/conv_epilogue.cuh); default 0
     lib.cd_conv_tc_set_staged_epilogue(int(os.environ['COLDDIFF_CONV_STAGED_EPILOGUE']))
-if os.environ.get('COLDDIFF_CONV_SIMT_PRELOAD') in ('0', '1'):   # image-edge kernels stage a chunk's receptive fields with all loads in flight; library default 1
-    lib.cd_conv_simt_set_preload(int(os.environ['COLDDIFF_CONV_SIMT_PRELOAD']))
-if os.environ.get('COLDDIFF_LAYERNORM_MULTI') in ('0', '2', '4'):   # C <= 128 LayerNorm forward with 2 / 4 pixels per lane group in flight (csrc/layernorm_multi.cu); library default 4
-    lib.cd_layernorm_set_multi(int(os.environ['COLDDIFF_LAYERNORM_MULTI']))
-if os.environ.get('COLDDIFF_LINATTN_STAGED') in ('0', '1'):   # shared-memory-staged cd_linattn_weff / cd_linattn_bwd_small (csrc/linattn_small.cu); library default 1
-    lib.cd_linattn_set_staged(int(os.environ['COLDDIFF_LINATTN_STAGED']))
 
 
 def _check(rc, what):
@@ -90,12 +84,12 @@ def ptr(t):
     return C.c_void_p(t.data_ptr())
 
 
-_LAUNCHES = {'cd_linattn_context': 2, 'cd_linattn_context_det': 2, 'cd_conv_wgrad': 2, 'cd_time_mlp_fwd': 2, 'cd_time_mlp2_fwd': 2, 'cd_version': 0, 'cd_last_error': 0}
+_LAUNCHES = {'cd_linattn_context_det': 2, 'cd_conv_wgrad': 2, 'cd_time_mlp_fwd': 2, 'cd_time_mlp2_fwd': 2, 'cd_version': 0, 'cd_last_error': 0}
 _launch_count = 0
 
 
 _PROF_SHAPE_ARGS = {'cd_dwconv7_fwd': (2, 3, 4, 5), 'cd_dwconv7_wgrad': (4, 5, 6, 7), 'cd_layernorm_bwd': (6, 7),
-                    'cd_layernorm_fwd': (2, 3), 'cd_linattn_context': (2, 3), 'cd_linattn_context_det': (2, 3), 'cd_linattn_bwd_kv': (2, 3)}
+                    'cd_layernorm_fwd': (2, 3), 'cd_linattn_context_det': (2, 3), 'cd_linattn_bwd_kv': (2, 3)}
 _prof = None          # tools/op_profile.py: list of (name, event0, event1) while profiling, else None
 
 

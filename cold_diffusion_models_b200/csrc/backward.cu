@@ -209,7 +209,7 @@ __global__ void colsum_batched_kernel(const float* __restrict__ x, int ld, long 
   }
 }
 
-// float4 variant (opt-in, the image-edge switch cd_conv_simt_set_preload; C % 4 == 0, 16-byte aligned rows): a warp covers 32/G rows x
+// float4 variant (C % 4 == 0, 16-byte aligned rows, rows >= 256; colsum_batched_kernel above serves the rest): a warp covers 32/G rows x
 // G channel quads (G = min(32, C/4) rounded up to a power of two), four independent 16-byte loads per thread in flight, partial
 // sums meet in shared memory, one atomicAdd per channel and block.  Different summation order than the scalar kernel: results agree to fp32 rounding.
 __global__ void __launch_bounds__(256)
@@ -316,12 +316,11 @@ attn_bwd_small_kernel(const float* __restrict__ dweff, const float* __restrict__
 constexpr int kKvPix = 32;
 constexpr int kKvTiles = 8;
 constexpr int kKvStride = 36;         // floats per channel row of the transposed tiles (16-byte aligned, 4-way store conflicts)
-// REMAP (opt-in, cd_linattn_set_staged): a warp owns ONE head and 4 pixel quads (lane = 8 channel quads x 4 pixel quads) instead of
-// all four heads of one pixel quad.  The heads' rows of every shared array are a multiple of 32 floats apart, so in the default
-// mapping the four heads of a warp hit the same banks: each of the four LDS.128 of a step costs 4 wavefronts (16 per 32 FMAs,
-// shared-memory bound at one wavefront per clock and SM); remapped, each is one 64- or 128-byte wavefront.  Same sums in the
-// same order -> bit-identical results.
-template <bool REMAP>
+// A warp owns ONE head and 4 pixel quads (lane = 8 channel quads x 4 pixel quads).  The heads' rows of every shared array are a
+// multiple of 32 floats apart, so a warp spanning the four heads of one pixel quad would hit the same banks: each of the four
+// LDS.128 of a step would cost 4 wavefronts (16 per 32 FMAs, shared-memory bound at one wavefront per clock and SM); with one
+// head per warp each is one 64- or 128-byte wavefront.
+// This CUDA-core kernel serves the operands the mma.sync kernel (linattn_bwd.cu) refuses: ld % 4 != 0 or unaligned qkv.
 __global__ void __launch_bounds__(256)
 attn_bwd_kv_kernel(const float* __restrict__ qkv, int ld, int n, const float* __restrict__ kmax,
                    const float* __restrict__ ksum, const float* __restrict__ dctxn, const float* __restrict__ rowdot,
@@ -339,10 +338,10 @@ attn_bwd_kv_kernel(const float* __restrict__ qkv, int ld, int n, const float* __
     dcA[i] = v;
     dcB[((hd & ~31) + e) * 32 + (hd & 31)] = v;
   }
-  // default: channel quad cq = lane (h = cq/8, j4 = (cq%8)*4), pixel quad = warp;  REMAP: head = warp % 4, pixel quad = 4 (warp / 4) + lane / 8
-  const int h = REMAP ? ((tid >> 5) & 3) : ((tid & 31) >> 3);
+  // head = warp % 4, channel quad j4 = lane % 8, pixel quad = 4 (warp / 4) + lane / 8
+  const int h = (tid >> 5) & 3;
   const int j4 = (tid & 7) * 4;
-  const int pq = REMAP ? ((tid >> 7) * 4 + ((tid & 31) >> 3)) : (tid >> 5);
+  const int pq = (tid >> 7) * 4 + ((tid & 31) >> 3);
   const int c4 = h * 32 + j4;
   const float4 rd = *reinterpret_cast<const float4*>(rowdot + b * 128 + c4);
   const int lc = tid & 127, lhalf = tid >> 7;
@@ -351,7 +350,7 @@ attn_bwd_kv_kernel(const float* __restrict__ qkv, int ld, int n, const float* __
     const int p0 = (blockIdx.x * tiles + tile) * kKvPix;
     if (p0 >= n) break;
     __syncthreads();                                 // previous tile consumed (and dc staged)
-    if constexpr (REMAP) {        // all 32 loads of the tile in flight before the first use (see context_kernel<PRELOAD>)
+    {                                                // all 32 loads of the tile in flight before the first use
       float kr[kKvPix / 2], vr[kKvPix / 2];
 #pragma unroll
       for (int u = 0; u < kKvPix / 2; ++u) {
@@ -369,17 +368,6 @@ attn_bwd_kv_kernel(const float* __restrict__ qkv, int ld, int n, const float* __
         psT[lc * kKvStride + pp] = (p0 + pp < n) ? __expf(kr[u] - kmx) * kinv : 0.f;
         vsT[lc * kKvStride + pp] = vr[u];
       }
-    } else {
-    for (int pp = lhalf; pp < kKvPix; pp += 2) {
-      const int p = p0 + pp;
-      float pv = 0.f, vv = 0.f;
-      if (p < n) {
-        const float* row = qkv + (static_cast<long long>(b) * n + p) * ld;
-        pv = __expf(row[128 + lc] - kmx) * kinv;
-        vv = row[256 + lc];
-      }
-      psT[lc * kKvStride + pp] = pv; vsT[lc * kKvStride + pp] = vv;
-    }
     }
     __syncthreads();
     float dk[4][4] = {}, dv[4][4] = {};               // [pixel][channel]
@@ -427,17 +415,17 @@ __global__ void transpose_weff_kernel(const float* __restrict__ w, int dim, floa
 // ---------------------------------------------------------------------------------------------
 // final 1x1 projection backward: dx[pix][c] = sum_co dout[b][co][pix] w[co][c]; dw[co][c], db[co]
 // ---------------------------------------------------------------------------------------------
-// thread = (pixel group, channel): x reads are coalesced over channels, dout is a warp broadcast
-// U = 4 (opt-in, the image-edge switch cd_conv_simt_set_preload): four pixels per trip with their loads issued first -- the default
-// keeps one 4-byte load per thread in flight (8 KB per SM) and is latency-bound at ~7x its HBM time.  Pixels are still consumed in
-// ascending order per thread, so every sum is formed in the same order.
+// thread = (pixel group, channel): x reads are coalesced over channels, dout is a warp broadcast.
+// Four pixels per trip with their loads issued first: one 4-byte load per thread in flight (8 KB per SM) left the kernel
+// latency-bound at ~7x its HBM time.  Pixels are consumed in ascending order per thread; the tail goes one pixel per trip.
 // CO > 0 fixes the number of image channels at compile time (3 for RGB): every per-channel array then lives in registers instead
-// of local memory (the run-time Co of the default instantiation indexes them dynamically).
-template <int U, int CO = 0>
+// of local memory (the run-time Co of the CO = 0 instantiation indexes them dynamically).
+template <int CO = 0>
 __global__ void __launch_bounds__(256)
 conv1x1_to_nchw_bwd_kernel(const float* __restrict__ dout, const float* __restrict__ x, int ld, int B, int HW, int C,
                            const float* __restrict__ w, int Co_rt, float* __restrict__ dx, int dx_ld,
                            float* __restrict__ dw, float* __restrict__ db, int pix_per_block) {
+  constexpr int U = 4;                // pixels per trip
   const int Co = CO > 0 ? CO : Co_rt;
   extern __shared__ float red[];      // [groups][Co][C]
   const int groups = blockDim.x / C;
@@ -449,31 +437,29 @@ conv1x1_to_nchw_bwd_kernel(const float* __restrict__ dout, const float* __restri
   for (int co = 0; co < Co; ++co) { wv[co] = w[co * C + c]; acc[co] = 0.f; accb[co] = 0.f; }
   if (gq < groups) {
     long long pix = p0 + gq;
-    if (U > 1) {
-      for (; pix + static_cast<long long>(U - 1) * groups < p1; pix += static_cast<long long>(U) * groups) {
-        float xv[U], dv[U][8];
+    for (; pix + static_cast<long long>(U - 1) * groups < p1; pix += static_cast<long long>(U) * groups) {
+      float xv[U], dv[U][8];
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const long long pu = pix + static_cast<long long>(u) * groups;
-          const int b = static_cast<int>(pu / HW), p = static_cast<int>(pu % HW);
-          xv[u] = x[pu * ld + c];
+      for (int u = 0; u < U; ++u) {
+        const long long pu = pix + static_cast<long long>(u) * groups;
+        const int b = static_cast<int>(pu / HW), p = static_cast<int>(pu % HW);
+        xv[u] = x[pu * ld + c];
 #pragma unroll
-          for (int co = 0; co < (CO > 0 ? CO : 8); ++co)
-            if (co < Co) dv[u][co] = dout[(static_cast<long long>(b) * Co + co) * HW + p];
-        }
+        for (int co = 0; co < (CO > 0 ? CO : 8); ++co)
+          if (co < Co) dv[u][co] = dout[(static_cast<long long>(b) * Co + co) * HW + p];
+      }
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-          float d = 0.f;
+      for (int u = 0; u < U; ++u) {
+        float d = 0.f;
 #pragma unroll
-          for (int co = 0; co < (CO > 0 ? CO : 8); ++co) {
-            if (co < Co) {
-              d = fmaf(dv[u][co], wv[co], d);
-              acc[co] = fmaf(dv[u][co], xv[u], acc[co]);
-              accb[co] += dv[u][co];
-            }
+        for (int co = 0; co < (CO > 0 ? CO : 8); ++co) {
+          if (co < Co) {
+            d = fmaf(dv[u][co], wv[co], d);
+            acc[co] = fmaf(dv[u][co], xv[u], acc[co]);
+            accb[co] += dv[u][co];
           }
-          dx[(pix + static_cast<long long>(u) * groups) * dx_ld + c] = d;
         }
+        dx[(pix + static_cast<long long>(u) * groups) * dx_ld + c] = d;
       }
     }
     for (; pix < p1; pix += groups) {
@@ -620,7 +606,7 @@ extern "C" int cd_dwconv7_wgrad(const float* dh, int dh_ld, const float* x, int 
 }
 
 extern "C" int cd_colsum_batched(const float* x, int ld, int B, int64_t rows, int C, float* out, int out_ld, void* stream) {
-  if (cd_conv_simt_preload_enabled() && C % 4 == 0 && ld % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && rows >= 256) {
+  if (C % 4 == 0 && ld % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && rows >= 256) {
     const int nq = C / 4;
     int G = 1; while (G < nq && G < 32) G <<= 1;
     const int xb = cd_cdiv(nq, G);
@@ -641,7 +627,7 @@ extern "C" int cd_colsum_batched(const float* x, int ld, int B, int64_t rows, in
 
 extern "C" int cd_linattn_bwd_small(const float* dweff, const float* ctx, const float* ksum, const float* w_out,
                                     int B, int dim, float scale, float* dw_out, float* dctxn, float* rowdot, void* stream) {
-  if (cd_linattn_staged_enabled(w_out, dweff))
+  if (cd_linattn_aligned(w_out, dweff))
     return cd_linattn_bwd_small_staged(dweff, ctx, ksum, w_out, B, dim, scale, dw_out, dctxn, rowdot, static_cast<cudaStream_t>(stream));
   attn_bwd_small_kernel<<<dim3(4, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(dweff, ctx, ksum, w_out, dim, scale, dw_out, dctxn, rowdot);
   CD_LAUNCH_CHECK();
@@ -653,13 +639,12 @@ extern "C" int cd_linattn_bwd_kv(const float* qkv, int ld, int B, int n, const f
   CD_REQUIRE(dld % 4 == 0 && (reinterpret_cast<uintptr_t>(dqkv) & 15) == 0, "cd_linattn_bwd_kv: dqkv must be 16-byte aligned with dld %% 4 == 0");
   {
     const int rc = cd_linattn_bwd_kv_mma(qkv, ld, B, n, kmax, ksum, dctxn, rowdot, dqkv, dld, static_cast<cudaStream_t>(stream));
-    if (rc <= 0) return rc;                      // 1: switch off (cd_linattn_set_bwd_mma) or unaligned operands -> CUDA-core kernel
+    if (rc <= 0) return rc;                      // 1: ld % 4 != 0 or unaligned qkv -> CUDA-core kernel
   }
   const size_t smem = sizeof(float) * (2 * 4096 + 2 * 128 * kKvStride);
   static bool attr = false;
   if (!attr) {
-    CD_CUDA(cudaFuncSetAttribute(attn_bwd_kv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CD_CUDA(cudaFuncSetAttribute(attn_bwd_kv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CD_CUDA(cudaFuncSetAttribute(attn_bwd_kv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = true;
   }
   // tiles per block: up to kKvTiles (amortises the 32 KB dctxn staging), fewer when that would leave SMs idle
@@ -667,10 +652,7 @@ extern "C" int cd_linattn_bwd_kv(const float* qkv, int ld, int B, int n, const f
   if (tiles > kKvTiles) tiles = kKvTiles;
   if (tiles < 1) tiles = 1;
   dim3 grid(cd_cdiv(n, kKvPix * tiles), B);
-  if (cd_linattn_staged_enabled(nullptr, nullptr))
-    attn_bwd_kv_kernel<true><<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(qkv, ld, n, kmax, ksum, dctxn, rowdot, dqkv, dld, tiles);
-  else
-    attn_bwd_kv_kernel<false><<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(qkv, ld, n, kmax, ksum, dctxn, rowdot, dqkv, dld, tiles);
+  attn_bwd_kv_kernel<<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(qkv, ld, n, kmax, ksum, dctxn, rowdot, dqkv, dld, tiles);
   CD_LAUNCH_CHECK();
   return 0;
 }
@@ -689,15 +671,12 @@ extern "C" int cd_conv1x1_to_nchw_bwd(const float* dout_nchw, const float* x, in
   const int groups = 256 / C;
   const size_t smem = sizeof(float) * size_t(groups) * Co * C;
   const int ppb = 1024;
-  if (cd_conv_simt_preload_enabled() && Co == 3)
-    conv1x1_to_nchw_bwd_kernel<4, 3><<<cd_cdiv(npix, ppb), 256, smem, static_cast<cudaStream_t>(stream)>>>(dout_nchw, x, ld, B, H * W, C, w, Co,
-                                                                                                         dx, dx_ld, dw, db, ppb);
-  else if (cd_conv_simt_preload_enabled())
-    conv1x1_to_nchw_bwd_kernel<4><<<cd_cdiv(npix, ppb), 256, smem, static_cast<cudaStream_t>(stream)>>>(dout_nchw, x, ld, B, H * W, C, w, Co,
+  if (Co == 3)
+    conv1x1_to_nchw_bwd_kernel<3><<<cd_cdiv(npix, ppb), 256, smem, static_cast<cudaStream_t>(stream)>>>(dout_nchw, x, ld, B, H * W, C, w, Co,
                                                                                                       dx, dx_ld, dw, db, ppb);
   else
-    conv1x1_to_nchw_bwd_kernel<1><<<cd_cdiv(npix, ppb), 256, smem, static_cast<cudaStream_t>(stream)>>>(dout_nchw, x, ld, B, H * W, C, w, Co,
-                                                                                                      dx, dx_ld, dw, db, ppb);
+    conv1x1_to_nchw_bwd_kernel<><<<cd_cdiv(npix, ppb), 256, smem, static_cast<cudaStream_t>(stream)>>>(dout_nchw, x, ld, B, H * W, C, w, Co,
+                                                                                                     dx, dx_ld, dw, db, ppb);
   CD_LAUNCH_CHECK();
   return 0;
 }

@@ -36,21 +36,21 @@ static inline int cd_num_sms() {
   return n;
 }
 
-// conv_simt.cu / final_proj.cu: opt-in variants of the image-edge kernels (cd_conv_simt_set_preload)
-int cd_conv_simt_preload_enabled();
+// final_proj.cu: the final 1x1 projection through a shared-memory tile; returns 1 when not taken
 int cd_conv1x1_to_nchw_tiled(const float* x, int ld, long long npix, int HW, int C, const float* w, const float* bias, int Co,
                              const float* resid, float* out, cudaStream_t st);
-// layernorm_multi.cu: C <= 128 LayerNorm forward with several pixels per lane group in flight (opt-in); returns 1 when not taken
+// layernorm_multi.cu: C <= 128 LayerNorm forward with several pixels per lane group in flight; returns 1 when not taken
 int cd_layernorm_fwd_multi(const float* x, int x_ld, long long npix, int C, const float* g, const float* beta, float eps,
                            float* y, int y_ld, float* stats, int round_tf32, cudaStream_t st);
-// linattn_small.cu: shared-memory-staged variants of the two per-(batch element, head) LinearAttention kernels (opt-in)
-int cd_linattn_staged_enabled(const void* a, const void* b);
+// linattn_small.cu: shared-memory-staged variants of the two per-(batch element, head) LinearAttention kernels, taken when
+// cd_linattn_aligned(a, b) (both pointers 16-byte aligned; a null pointer counts as aligned)
+int cd_linattn_aligned(const void* a, const void* b);
 int cd_linattn_weff_staged(const float* ctx, const float* ksum, const float* w_out, int B, int dim, float scale,
                            int round_tf32, float* weff, cudaStream_t st);
 int cd_linattn_bwd_small_staged(const float* dweff, const float* ctx, const float* ksum, const float* w_out, int B, int dim,
                                 float scale, float* dw_out, float* dctxn, float* rowdot, cudaStream_t st);
 
-// linattn_bwd.cu: per-pixel LinearAttention backward on mma.sync (default); returns 1 when the CUDA-core kernel should run
+// linattn_bwd.cu: per-pixel LinearAttention backward on mma.sync; returns 1 when the CUDA-core kernel should run
 int cd_linattn_bwd_kv_mma(const float* qkv, int ld, int B, int n, const float* kmax, const float* ksum, const float* dctxn,
                           const float* rowdot, float* dqkv, int dld, cudaStream_t st);
 

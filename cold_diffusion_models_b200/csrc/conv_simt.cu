@@ -151,10 +151,9 @@ conv_smallc_kernel(const SimtParams p) {
 // K = ntaps*C weights in registers; 256 threads cover 256/(Cout/4) pixels at a time, the receptive fields of a 64-pixel
 // chunk are staged in shared memory and read as broadcast LDS.128; a warp writes whole contiguous output rows.
 // (16*KQ FMAs per KQ LDS.128 instead of 4 per LDS.128, and coalesced stores instead of one pixel row per thread.)
-// opt-in (cd_conv_simt_set_preload): the register-tiled image-edge kernels run ONE block of 8 warps per SM (~185-227 registers per
-// thread), so nothing hides the memory latency of the staging loop below; with the switch on, the (at most three) receptive-field
-// entries a thread stages per 64-pixel chunk are all loaded before the first one is stored.  Same values in the same places.
-static int g_simt_preload = 1;
+// The register-tiled image-edge kernels run ONE block of 8 warps per SM (~185-227 registers per thread), so nothing hides the
+// memory latency of a staging loop; stage_patches_preload loads the (at most three) receptive-field entries a thread stages per
+// 64-pixel chunk before it stores the first one.  stage_patches (same values in the same places) serves tap counts above 12.
 __device__ __forceinline__ void stage_patches_preload(float* patch_f, int KP, long long q0, long long pend, const float* __restrict__ src,
                                                       int ld, int C, int H, int W, int Hg, int Wg, int sy, int sx, int ntaps,
                                                       const int* dyv, const int* dxv) {
@@ -696,7 +695,7 @@ static int conv_fwd_simt(const CdConvDesc* d, cudaStream_t st) {
       const int cpb = cd_cdiv(chunks, blocks);
       const int grid = cd_cdiv(chunks, cpb);
       const int KQ = cd_cdiv(c0.ntaps * c0.C, 4);
-      const int pre = (g_simt_preload && 64 * c0.ntaps <= 768) ? 1 : 0;
+      const int pre = 64 * c0.ntaps <= 768 ? 1 : 0;
       if (KQ <= 1) conv_smallc4_kernel<1><<<grid, 256, 0, st>>>(p, cpb, pre);
       else if (KQ <= 3) conv_smallc4_kernel<3><<<grid, 256, 0, st>>>(p, cpb, pre);
       else if (KQ <= 7) conv_smallc4_kernel<7><<<grid, 256, 0, st>>>(p, cpb, pre);
@@ -756,7 +755,7 @@ extern "C" int cd_conv_wgrad(const CdConvDesc* d, const float* dout, int dout_ld
     p.pix_per_split = cd_cdiv(total, blocks);
     const int grid = cd_cdiv(total, p.pix_per_split);
     const int KQ = cd_cdiv(Ksm, 4);
-    const int wpre = (g_simt_preload && 64 * c.ntaps <= 768) ? 1 : 0;
+    const int wpre = 64 * c.ntaps <= 768 ? 1 : 0;
     if (KQ <= 1) wgrad_smallc4_kernel<1><<<grid, 256, 0, st>>>(p, wpre);
     else if (KQ <= 3) wgrad_smallc4_kernel<3><<<grid, 256, 0, st>>>(p, wpre);
     else if (KQ <= 7) wgrad_smallc4_kernel<7><<<grid, 256, 0, st>>>(p, wpre);
@@ -799,9 +798,6 @@ extern "C" int cd_conv_wgrad(const CdConvDesc* d, const float* dout, int dout_ld
   }
   return 0;
 }
-
-extern "C" int cd_conv_simt_set_preload(int enable) { g_simt_preload = enable ? 1 : 0; return 0; }
-int cd_conv_simt_preload_enabled() { return g_simt_preload; }
 
 extern "C" int cd_colsum(const float* x, int ld, int64_t rows, int C, float* out, void* stream) {
   launch_colsum(x, ld, rows, C, out, static_cast<cudaStream_t>(stream));

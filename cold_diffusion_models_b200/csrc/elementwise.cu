@@ -562,96 +562,8 @@ cond_proj_kernel(const float* __restrict__ temb, int dim, const float* __restric
 }
 
 // ---------------------------------------------------------------------------------------------
-// LinearAttention: k-softmax statistics and context.  qkv NHWC [B][n][ld], q|k|v at 0|128|256.
+// LinearAttention: effective output weights from the context (linattn_ctx.cu computes kmax / ksum / ctx).
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void atomic_max_float(float* addr, float v) {
-  // valid for any sign mix: positive floats order as ints, negative floats order reversed as uints
-  if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
-  else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
-}
-
-__global__ void __launch_bounds__(256)
-kmax_kernel(const float* __restrict__ qkv, int ld, int n, int pix_per_block, float* __restrict__ kmax) {
-  const int b = blockIdx.y;
-  const int c = threadIdx.x & 127, half = threadIdx.x >> 7;
-  const int p0 = blockIdx.x * pix_per_block;
-  int p1 = p0 + pix_per_block; if (p1 > n) p1 = n;
-  float m = -INFINITY;
-  for (int p = p0 + half; p < p1; p += 2) m = fmaxf(m, qkv[(static_cast<long long>(b) * n + p) * ld + 128 + c]);
-  atomic_max_float(kmax + b * 128 + c, m);
-}
-
-constexpr int kCtxP = 32;   // pixels per smem chunk
-// PRELOAD (opt-in, cd_linattn_set_staged): the 16 k and 16 v values a thread stages per chunk are all requested before the first
-// exp / store instead of one dependent load -> exp -> store round trip per pixel (the loop is not unrolled by the compiler because of
-// its bounds check: ~16 exposed memory latencies per chunk).  Same values, same order of the ksum partial sums.
-template <bool PRELOAD>
-__global__ void __launch_bounds__(256)
-context_kernel(const float* __restrict__ qkv, int ld, int n, int pix_per_block, const float* __restrict__ kmax,
-               float* __restrict__ ksum, float* __restrict__ ctx) {
-  __shared__ float es[kCtxP][128];
-  __shared__ float vs[kCtxP][128];
-  const int b = blockIdx.y;
-  const int p0 = blockIdx.x * pix_per_block;
-  int p1 = p0 + pix_per_block; if (p1 > n) p1 = n;
-  const int tid = threadIdx.x;
-  const int h = tid >> 6, d4 = ((tid & 63) >> 3) * 4, e4 = (tid & 7) * 4;
-  const int lc = tid & 127, lhalf = tid >> 7;
-  const float mx = kmax[b * 128 + lc];
-  float acc[4][4] = {};
-  float esum = 0.f;
-  for (int q0 = p0; q0 < p1; q0 += kCtxP) {
-    if constexpr (PRELOAD) {
-      float kr[kCtxP / 2], vr[kCtxP / 2];
-#pragma unroll
-      for (int u = 0; u < kCtxP / 2; ++u) {
-        const int p = q0 + lhalf + 2 * u;
-        kr[u] = 0.f; vr[u] = 0.f;
-        if (p < p1) {
-          const float* row = qkv + (static_cast<long long>(b) * n + p) * ld;
-          kr[u] = row[128 + lc];
-          vr[u] = row[256 + lc];
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < kCtxP / 2; ++u) {
-        const int pp = lhalf + 2 * u;
-        const float e = (q0 + pp < p1) ? __expf(kr[u] - mx) : 0.f;
-        es[pp][lc] = e; vs[pp][lc] = vr[u]; esum += e;
-      }
-    } else {
-    for (int pp = lhalf; pp < kCtxP; pp += 2) {
-      const int p = q0 + pp;
-      float e = 0.f, v = 0.f;
-      if (p < p1) {
-        const float* row = qkv + (static_cast<long long>(b) * n + p) * ld;
-        e = __expf(row[128 + lc] - mx);
-        v = row[256 + lc];
-      }
-      es[pp][lc] = e; vs[pp][lc] = v; esum += e;
-    }
-    }
-    __syncthreads();
-#pragma unroll 4
-    for (int pp = 0; pp < kCtxP; ++pp) {
-      const float4 ev = *reinterpret_cast<const float4*>(&es[pp][h * 32 + d4]);
-      const float4 vv = *reinterpret_cast<const float4*>(&vs[pp][h * 32 + e4]);
-      const float e[4] = {ev.x, ev.y, ev.z, ev.w}, v[4] = {vv.x, vv.y, vv.z, vv.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(e[i], v[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-  atomicAdd(ksum + b * 128 + lc, esum);
-  float* cb = ctx + (static_cast<long long>(b) * 4 + h) * 1024;
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) atomicAdd(cb + (d4 + i) * 32 + e4 + j, acc[i][j]);
-}
-
 // weff[b][co][h*32+d] = scale * sum_e w_out[co][h*32+e] * ctx[b][h][d][e] / ksum[b][h*32+d]
 // block = (head, batch element): the normalised 32x32 context is staged in shared memory.
 __global__ void __launch_bounds__(256)
@@ -741,7 +653,7 @@ extern "C" int cd_layernorm_fwd(const float* x, int x_ld, int64_t npix, int C, c
   const int blocks = cd_cdiv(npix, 8 * ppw);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (slots == 1 && g != nullptr && beta != nullptr) {
-    const int rc = cd_layernorm_fwd_multi(x, x_ld, npix, C, g, beta, eps, y, y_ld, stats, round_tf32, st);   // opt-in, layernorm_multi.cu
+    const int rc = cd_layernorm_fwd_multi(x, x_ld, npix, C, g, beta, eps, y, y_ld, stats, round_tf32, st);   // layernorm_multi.cu
     if (rc <= 0) return rc;
   }
 #define CD_LNF(N) layernorm_kernel<N><<<blocks, 256, 0, st>>>(x, x_ld, npix, C, g, beta, eps, y, y_ld, stats, round_tf32)
@@ -834,50 +746,9 @@ extern "C" int cd_time_mlp_fwd(const int64_t* t, int B, int dim, const float* w1
   return 0;
 }
 
-extern "C" int cd_linattn_context(const float* qkv, int ld, int B, int n, float* kmax, float* ksum, float* ctx,
-                                  void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // kmax starts at -inf, ksum/ctx at zero (async memsets: stream-ordered and graph-capturable)
-  CD_CUDA(cudaMemsetAsync(ksum, 0, sizeof(float) * B * 128, st));
-  CD_CUDA(cudaMemsetAsync(ctx, 0, sizeof(float) * B * 4096, st));
-  {
-    typedef CUresult (*MemsetD32Async)(CUdeviceptr, unsigned int, size_t, CUstream);
-    static MemsetD32Async fn = nullptr;
-    if (!fn) {
-      void* p = nullptr; cudaDriverEntryPointQueryResult q;
-      if (cudaGetDriverEntryPoint("cuMemsetD32Async", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-        fn = reinterpret_cast<MemsetD32Async>(p);
-    }
-    CD_REQUIRE(fn != nullptr, "cuMemsetD32Async unavailable");
-    CD_REQUIRE(fn(reinterpret_cast<CUdeviceptr>(kmax), 0xFF800000u, static_cast<size_t>(B) * 128, st) == CUDA_SUCCESS,
-               "cuMemsetD32Async failed");
-  }
-  // pixels per block: one wave of resident blocks over the whole batch (a fixed 512 left the 64x64 level with 256 blocks
-  // and the 128x128 level with 1.15 waves); any value is correct, the kernels clamp to n and zero-fill the last chunk
-  const int variant = cd_linattn_staged_enabled(nullptr, nullptr) ? 1 : 0;     // the PRELOAD kernel holds 32 more registers
-  static int slots_v[2] = {0, 0};
-  if (!slots_v[variant]) {
-    int occ = 0;
-    if (variant) CD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, context_kernel<true>, 256, 0));
-    else CD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, context_kernel<false>, 256, 0));
-    slots_v[variant] = cd_num_sms() * (occ > 0 ? occ : 1);
-  }
-  const int slots = slots_v[variant];
-  int per_img = slots / (B > 0 ? B : 1); if (per_img < 1) per_img = 1;
-  int ppb = cd_cdiv(cd_cdiv(n, per_img), kCtxP) * kCtxP;
-  if (ppb < kCtxP) ppb = kCtxP;
-  dim3 grid(cd_cdiv(n, ppb), B);
-  kmax_kernel<<<grid, 256, 0, st>>>(qkv, ld, n, ppb, kmax);
-  CD_LAUNCH_CHECK();
-  if (variant) context_kernel<true><<<grid, 256, 0, st>>>(qkv, ld, n, ppb, kmax, ksum, ctx);
-  else context_kernel<false><<<grid, 256, 0, st>>>(qkv, ld, n, ppb, kmax, ksum, ctx);
-  CD_LAUNCH_CHECK();
-  return 0;
-}
-
 extern "C" int cd_linattn_weff(const float* ctx, const float* ksum, const float* w_out, int B, int dim, float scale,
                                int round_tf32, float* weff, void* stream) {
-  if (cd_linattn_staged_enabled(w_out, nullptr))
+  if (cd_linattn_aligned(w_out, nullptr))
     return cd_linattn_weff_staged(ctx, ksum, w_out, B, dim, scale, round_tf32, weff, static_cast<cudaStream_t>(stream));
   weff_kernel<<<dim3(4, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(ctx, ksum, w_out, dim, scale, round_tf32, weff);
   CD_LAUNCH_CHECK();
@@ -888,7 +759,7 @@ extern "C" int cd_conv1x1_to_nchw(const float* x, int ld, int B, int H, int W, i
                                   const float* b, int Co, const float* resid_nchw, float* out_nchw, void* stream) {
   CD_REQUIRE(C % 4 == 0 && ld % 4 == 0, "cd_conv1x1_to_nchw: C must be a multiple of 4");
   const long long npix = static_cast<long long>(B) * H * W;
-  if (cd_conv_simt_preload_enabled()) {                  // opt-in: tile through shared memory (final_proj.cu)
+  {                                                      // tile through shared memory (final_proj.cu) where eligible
     const int rc = cd_conv1x1_to_nchw_tiled(x, ld, npix, H * W, C, w, b, Co, resid_nchw, out_nchw, static_cast<cudaStream_t>(stream));
     if (rc <= 0) return rc;
   }

@@ -1,10 +1,10 @@
-// Final 1x1 projection to image channels (NHWC features -> NCHW image, DB:253,279-282) through a shared-memory tile (opt-in, the
-// image-edge switch cd_conv_simt_set_preload).  conv1x1_to_nchw_kernel (elementwise.cu) gives every thread one pixel and lets it
+// Final 1x1 projection to image channels (NHWC features -> NCHW image, DB:253,279-282) through a shared-memory tile, for C = 32,
+// 64 or 128.  conv1x1_to_nchw_kernel (elementwise.cu; the other C) gives every thread one pixel and lets it
 // read its own 256-byte feature row with float4 loads: each warp instruction touches 32 different lines (the row-per-lane pattern
 // that bounds the row epilogue of the tensor-core convolutions) and the row is read again for every output channel.  Here the
 // 128 x C tile of a block is loaded with line-coalesced float4 loads (the rows of consecutive pixels are adjacent in memory when
 // ld == C), each thread then takes its pixel's row from shared memory (row stride C + 1: conflict-free) into registers once and
-// forms the Co dot products in the SAME order as the default kernel (bias first, channels ascending) -> bit-identical.
+// forms the Co dot products in the SAME order as conv1x1_to_nchw_kernel (bias first, channels ascending) -> bit-identical.
 #include "cd_common.cuh"
 
 namespace {

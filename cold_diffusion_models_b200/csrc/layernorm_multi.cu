@@ -1,15 +1,14 @@
-// Channel LayerNorm forward for C <= 128 with PP pixels per lane group in flight (opt-in, cd_layernorm_set_multi).
-// layernorm_kernel<1> (elementwise.cu) gives every thread ONE float4 load before two shuffle reductions: 2048 resident threads x 16
-// bytes = 32 KB in flight per SM, about what HBM latency x bandwidth needs.  Here a lane group loads PP pixels up front (PP x 16 bytes per thread in flight), then normalises them
-// with the same per-pixel arithmetic in the same order (sum over the group by xor-shuffles, mean, centred sum of squares, rstd) --
-// bit-identical results.
+// Channel LayerNorm forward for C <= 128 (C / 4 a power of two) with PP = 4 pixels per lane group in flight, on 4096 pixels or more.
+// layernorm_kernel<1> (elementwise.cu), which serves the other shapes, gives every thread ONE float4 load before two shuffle
+// reductions: 2048 resident threads x 16 bytes = 32 KB in flight per SM, about what HBM latency x bandwidth needs.  Here a lane
+// group loads PP pixels up front (PP x 16 bytes per thread in flight), then normalises them with the same per-pixel arithmetic in
+// the same order (sum over the group by xor-shuffles, mean, centred sum of squares, rstd) -- bit-identical results.
 #include "cd_common.cuh"
 
 namespace {
 
-int g_ln_multi = 4;
+constexpr int PP = 4;                 // pixels per lane group
 
-template <int PP>
 __global__ void __launch_bounds__(256)
 layernorm_multi_kernel(const float* __restrict__ x, int x_ld, long long npix, int C, const float* __restrict__ g,
                        const float* __restrict__ beta, float eps, float* __restrict__ y, int y_ld,
@@ -57,19 +56,13 @@ layernorm_multi_kernel(const float* __restrict__ x, int x_ld, long long npix, in
 
 }  // namespace
 
-extern "C" int cd_layernorm_set_multi(int pixels_per_group) { g_ln_multi = pixels_per_group; return 0; }
-
-// 1: not taken (switch off or shape not eligible) -> the caller launches layernorm_kernel<1>
+// 1: shape not eligible -> the caller launches layernorm_kernel<N>
 int cd_layernorm_fwd_multi(const float* x, int x_ld, long long npix, int C, const float* g, const float* beta, float eps,
                            float* y, int y_ld, float* stats, int round_tf32, cudaStream_t st) {
   const int nq = C / 4;
-  if (g_ln_multi < 2 || nq > 32 || (nq & (nq - 1)) != 0 || npix < 4096) return 1;
+  if (nq > 32 || (nq & (nq - 1)) != 0 || npix < 4096) return 1;
   const int ppw = 32 / nq;
-  if (g_ln_multi >= 4) {
-    layernorm_multi_kernel<4><<<cd_cdiv(npix, 8 * ppw * 4), 256, 0, st>>>(x, x_ld, npix, C, g, beta, eps, y, y_ld, stats, round_tf32);
-  } else {
-    layernorm_multi_kernel<2><<<cd_cdiv(npix, 8 * ppw * 2), 256, 0, st>>>(x, x_ld, npix, C, g, beta, eps, y, y_ld, stats, round_tf32);
-  }
+  layernorm_multi_kernel<<<cd_cdiv(npix, 8 * ppw * PP), 256, 0, st>>>(x, x_ld, npix, C, g, beta, eps, y, y_ld, stats, round_tf32);
   CD_LAUNCH_CHECK();
   return 0;
 }

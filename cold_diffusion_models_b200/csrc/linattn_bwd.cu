@@ -145,16 +145,12 @@ attn_bwd_kv_mma_kernel(const float* __restrict__ qkv, int ld, int n, int ppb, co
   }
 }
 
-int g_bwd_mma = 1;
-
 }  // namespace
 
-extern "C" int cd_linattn_set_bwd_mma(int enable) { g_bwd_mma = enable ? 1 : 0; return 0; }
-
-// returns 1 when the caller should use the CUDA-core kernel (switch off or unaligned operands)
+// returns 1 when the caller should use the CUDA-core kernel (ld % 4 != 0 or unaligned operands)
 int cd_linattn_bwd_kv_mma(const float* qkv, int ld, int B, int n, const float* kmax, const float* ksum, const float* dctxn,
                           const float* rowdot, float* dqkv, int dld, cudaStream_t st) {
-  if (!g_bwd_mma || ld % 4 != 0 || dld % 2 != 0 || (reinterpret_cast<uintptr_t>(qkv) & 15) != 0 || (reinterpret_cast<uintptr_t>(dqkv) & 7) != 0)
+  if (ld % 4 != 0 || dld % 2 != 0 || (reinterpret_cast<uintptr_t>(qkv) & 15) != 0 || (reinterpret_cast<uintptr_t>(dqkv) & 7) != 0)
     return 1;
   const size_t smem = sizeof(float) * (2 * 4 * 32 * kLc + 3 * 128 + 2 * 2 * kP * kLd);
   static bool attr = false;

@@ -3,9 +3,9 @@
 //
 //   ctx[b][h][d][e] = sum_n exp(k[b][n][h*32+d] - kmax[b][h*32+d]) * v[b][n][h*32+e],   ksum[b][c] = sum_n exp(k[b][n][c] - kmax[b][c])
 //
-// A max pass, a CUDA-core outer-product pass and float atomics over the pixel blocks (cd_linattn_context) read k twice and give
-// a result whose last bit depends on the order of the atomics -- which the TF32 roundings downstream amplify into run-to-run
-// differences of the network output.
+// A max pass, a CUDA-core outer-product pass and float atomics over the pixel blocks would read k twice and give a result whose
+// last bit depends on the order of the atomics -- which the TF32 roundings downstream amplify into run-to-run differences of the
+// network output.
 //
 // Here a block walks a contiguous span of pixels of one image with the flash-attention recurrence: running per-channel max m,
 // accumulators rescaled by exp(m_old - m_new) when m grows.  The 32x32 (per head) products E^T V run on the tensor cores with

@@ -3,14 +3,12 @@
 // output channels with dependent strided global loads: a few MFLOP per call, bound by load latency.  The kernels below read
 // every operand once, 64 channel rows per pass with all loads of a pass in flight (one float4 per thread and array), and keep
 // the arithmetic ORDER of the originals (sums over co / d / e ascending, one fmaf per term), so their results are bit-identical
-// up to the order of the float atomics that were already there.
-// The same switch selects the bank-conflict-free thread mapping of attn_bwd_kv_kernel<REMAP> (backward.cu).
-// Switch: cd_linattn_set_staged(1) / COLDDIFF_LINATTN_STAGED=1.
+// up to the order of the float atomics that were already there.  The originals serve a w_out (weff) or dweff (backward) that is
+// not 16-byte aligned.
 #include "cd_common.cuh"
 
 namespace {
 
-int g_staged = 1;
 constexpr int kRows = 64;            // channel rows (co) staged per pass
 
 // weff[b][co][h*32+d] = sum_e w_out[co][h*32+e] * ctxn[d][e],  ctxn[d][e] = ctx[b][h][d][e] * scale / ksum[b][h*32+d]
@@ -109,11 +107,9 @@ attn_bwd_small_staged_kernel(const float* __restrict__ dweff, const float* __res
 }  // namespace
 
 // the staged kernels read rows with float4 loads: callers fall back to the original kernels for unaligned operands
-int cd_linattn_staged_enabled(const void* a, const void* b) {
-  return g_staged && ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0;
+int cd_linattn_aligned(const void* a, const void* b) {
+  return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0;
 }
-
-extern "C" int cd_linattn_set_staged(int enable) { g_staged = enable ? 1 : 0; return 0; }
 
 int cd_linattn_weff_staged(const float* ctx, const float* ksum, const float* w_out, int B, int dim, float scale,
                            int round_tf32, float* weff, cudaStream_t st) {

@@ -164,21 +164,19 @@ int cd_time_mlp_fwd(const int64_t* t, int B, int dim, const float* w1, const flo
                     float* cond_all /*[B][sumC]*/, void* stream);
 
 /* LinearAttention core (DB:176-187) on qkv NHWC [B][n][ld] (q|k|v at channel 0|128|256, 4 heads x 32):
+ *   kmax[b,h,d]   = max_n k[b,h,d,n]
  *   ctx[b,h,d,e]  = sum_n exp(k[b,h,d,n] - kmax[b,h,d]) * v[b,h,e,n]      (un-normalised)
  *   ksum[b,h,d]   = sum_n exp(k[b,h,d,n] - kmax[b,h,d])
  *   weff[b, co, h*32+d] = scale * sum_e w_out[co, h*32+e] * ctx[b,h,d,e] / ksum[b,h,d]
  * so that to_out(einsum(context, q*scale)) == conv1x1(q, weff[b]) -- a per-batch-weight tap-list
  * convolution (cd_conv_fwd with w_per_batch=1).  kmax/ksum ([B][128]) are kept for backward. */
-int cd_linattn_context(const float* qkv, int ld, int B, int n, float* kmax, float* ksum,
-                       float* ctx /*[B][4][32][32]*/, void* stream);
 int cd_linattn_weff(const float* ctx, const float* ksum, const float* w_out /*[dim][128]*/, int B, int dim,
                     float scale, int round_tf32, float* weff /*[B][dim][128]*/, void* stream);
-/* The same kmax / ksum / ctx as cd_linattn_context, DETERMINISTIC (bit-identical run to run) and in one pass over k and v
+/* kmax / ksum / ctx as above, DETERMINISTIC (bit-identical run to run) and in one pass over k and v
  * (csrc/linattn_ctx.cu): blocks walk spans of `ppb` pixels with a running max (flash-attention recurrence), the per-head E^T V
  * products run as 3xTF32 mma.sync, each block writes one partial (ctx[4][32][32] | m[128] | s[128] = 4352 floats) to `ws`
  * ([B][nblk][4352] floats, caller-allocated) and a second kernel merges the partials of an image in block order.
- * The caller picks ppb (a multiple of 32; about one wave of blocks at 3 blocks per SM over the batch) and nblk = ceil(n / ppb).
- * This is what the engine calls; cd_linattn_context (float atomics) stays for A/B comparisons. */
+ * The caller picks ppb (a multiple of 32; about one wave of blocks at 3 blocks per SM over the batch) and nblk = ceil(n / ppb). */
 int cd_linattn_context_det(const float* qkv, int ld, int B, int n, int nblk, int ppb, float* ws, float* kmax, float* ksum,
                            float* ctx /*[B][4][32][32]*/, void* stream);
 
@@ -206,17 +204,6 @@ int cd_conv_fwd_f16_probe(const CdConvDesc* d, void* stream);
  * bit-identical results): 1 = for launches with at most 16 K chunks of 32 channels per tile (the store-bound 1x1 projections),
  * 2 = for every launch, 3 = at most 48 K chunks */
 int cd_conv_tc_set_staged_epilogue(int mode);
-/* opt-in (default 0): the register-tiled image-edge convolution / weight-gradient kernels (Cin <= 4)
- * load all receptive-field entries of a 64-pixel chunk before storing the first (csrc/conv_simt.cu: stage_patches_preload), and
- * cd_conv1x1_to_nchw goes through a shared-memory tile (csrc/final_proj.cu), cd_conv1x1_to_nchw_bwd keeps four pixels per trip in
- * flight and cd_colsum_batched uses float4 loads (csrc/backward.cu): more bytes in flight, same arithmetic */
-int cd_conv_simt_set_preload(int enable);
-/* opt-in (default 0): channel LayerNorm forward for C <= 128 with 2 or 4 pixels per lane group in
- * flight (csrc/layernorm_multi.cu; same per-pixel arithmetic) */
-int cd_layernorm_set_multi(int pixels_per_group);
-/* opt-in (default 0): shared-memory-staged kernels behind cd_linattn_weff / cd_linattn_bwd_small
- * (csrc/linattn_small.cu; same arithmetic order as the default kernels) */
-int cd_linattn_set_staged(int enable);
 /* diagnostic switch: 1 (default) = TFLOAT32 tensor maps, 0 = FLOAT32 tensor maps for the convolution operands */
 int cd_conv_tc_set_tf32_maps(int enable);
 /* SM-pair variant of the tap-list convolution: a cluster of two CTAs computes two neighbouring 128-pixel tiles of the same output
@@ -247,14 +234,13 @@ int cd_dwconv7_wgrad(const float* dh, int dh_ld, const float* x, int x_ld, int B
                      float* dw, void* stream);
 /* out[b*out_ld + c] += sum over the `rows` pixels of image b of x[.., c]  (time-conditioning gradient) */
 int cd_colsum_batched(const float* x, int ld, int B, int64_t rows, int C, float* out, int out_ld, void* stream);
-/* LinearAttention backward (see cd_linattn_context): per-batch small part and per-pixel k/v part */
+/* LinearAttention backward (see cd_linattn_context_det): per-batch small part and per-pixel k/v part */
 int cd_linattn_bwd_small(const float* dweff, const float* ctx, const float* ksum, const float* w_out,
                          int B, int dim, float scale, float* dw_out, float* dctxn, float* rowdot, void* stream);
+/* cd_linattn_bwd_kv runs its two [pixels x 32] x [32 x 32] products per head on warp-level tensor-core MMAs (csrc/linattn_bwd.cu:
+ * 3xTF32: fp32-grade products); ld % 4 != 0 or a qkv that is not 16-byte aligned takes a CUDA-core kernel */
 int cd_linattn_bwd_kv(const float* qkv, int ld, int B, int n, const float* kmax, const float* ksum,
                       const float* dctxn, const float* rowdot, float* dqkv, int dld, void* stream);
-/* cd_linattn_bwd_kv runs its two [pixels x 32] x [32 x 32] products per head on warp-level tensor-core MMAs (csrc/linattn_bwd.cu:
- * 3xTF32: fp32-grade products); 0 selects the CUDA-core kernel (A/B comparisons) */
-int cd_linattn_set_bwd_mma(int enable);
 int cd_transpose_weff(const float* weff, int B, int dim, float* weff_t, void* stream);
 int cd_conv1x1_to_nchw_bwd(const float* dout_nchw, const float* x, int ld, int B, int H, int W, int C,
                            const float* w, int Co, float* dx, int dx_ld, float* dw, float* db, void* stream);

@@ -1,6 +1,7 @@
 """GPU parity of the API helpers (Individual_Incremental, resolution Step routine / t = -1 rows, sample_from_blur, all_sample /
-forward_and_backward of every package, Unet constructor options, the evaluation routines) against the reference goldens, and of
-the kernel variants behind library switches against the kernels they replace."""
+forward_and_backward of every package, Unet constructor options, the evaluation routines) against the reference goldens, of
+the kernel variants behind library switches against the kernels they replace, and of the memory-bound kernels of the
+LinearAttention, LayerNorm and image edge against float64."""
 import io
 import contextlib
 import pytest
@@ -244,10 +245,18 @@ def test_batched_repack_matches_the_single_launches():
         assert rel(grads[1][n], grads[0][n]) < 2e-3, n
 
 
-@OPT_IN
-def test_linattn_staged_kernels_match_the_default_ones():
-    """csrc/linattn_small.cu (cd_linattn_set_staged / COLDDIFF_LINATTN_STAGED): same arithmetic order as the default kernels, so weff / dctxn / rowdot are bit-identical and dW_out (float atomics over
-    the batch) agrees to rounding"""
+def _unaligned(t):
+    """a copy of `t` whose data starts 4 bytes past a 16-byte boundary (selects the kernels that take any alignment)"""
+    u = torch.empty(t.numel() + 1, dtype=t.dtype, device=t.device)[1:].view(t.shape)
+    u.copy_(t)
+    assert u.data_ptr() % 16 != 0
+    return u
+
+
+def test_linattn_kernels_against_float64():
+    """LinearAttention entry points against float64 torch: cd_linattn_weff / cd_linattn_bwd_small (shared-memory-staged kernels of
+    csrc/linattn_small.cu, bit-identical to the kernels that serve an unaligned w_out / dweff), cd_linattn_bwd_kv (tensor-core kernel, and
+    the CUDA-core kernel for ld % 4 != 0) and cd_linattn_context_det"""
     import ctypes as C
     from cold_diffusion_models_b200._lib import lib, ptr, stream, _check
     gen = torch.Generator().manual_seed(3)
@@ -255,57 +264,62 @@ def test_linattn_staged_kernels_match_the_default_ones():
         ctx, ksum = torch.randn(B, 4, 32, 32, generator=gen).cuda(), (1 + 30 * torch.rand(B, 128, generator=gen)).cuda()
         w_out, dweff = (torch.randn(dim, 128, generator=gen) / 11).cuda(), torch.randn(B, dim, 128, generator=gen).cuda()
         res = []
-        try:
-            for staged in (0, 1):
-                lib.cd_linattn_set_staged(staged)
-                weff = [torch.full((B, dim, 128), 7.0).cuda() for _ in range(2)]
-                for rnd in (0, 1):
-                    _check(lib.cd_linattn_weff(ptr(ctx), ptr(ksum), ptr(w_out), B, dim, C.c_float(0.17), rnd, ptr(weff[rnd]), stream()), 'weff')
-                dw_out, dctxn, rowdot = torch.zeros(dim, 128).cuda(), torch.full((B, 4, 32, 32), 7.0).cuda(), torch.full((B, 128), 7.0).cuda()
-                _check(lib.cd_linattn_bwd_small(ptr(dweff), ptr(ctx), ptr(ksum), ptr(w_out), B, dim, C.c_float(0.17), ptr(dw_out), ptr(dctxn),
-                                                ptr(rowdot), stream()), 'bwd_small')
-                torch.cuda.synchronize()
-                res.append((weff[0], weff[1], dctxn, rowdot, dw_out))
-        finally:
-            lib.cd_linattn_set_staged(0)
+        for wo, dwe in ((w_out, dweff), (_unaligned(w_out), _unaligned(dweff))):
+            weff = [torch.full((B, dim, 128), 7.0).cuda() for _ in range(2)]
+            for rnd in (0, 1):
+                _check(lib.cd_linattn_weff(ptr(ctx), ptr(ksum), ptr(wo), B, dim, C.c_float(0.17), rnd, ptr(weff[rnd]), stream()), 'weff')
+            dw_out, dctxn, rowdot = torch.zeros(dim, 128).cuda(), torch.full((B, 4, 32, 32), 7.0).cuda(), torch.full((B, 128), 7.0).cuda()
+            _check(lib.cd_linattn_bwd_small(ptr(dwe), ptr(ctx), ptr(ksum), ptr(w_out), B, dim, C.c_float(0.17), ptr(dw_out), ptr(dctxn),
+                                            ptr(rowdot), stream()), 'bwd_small')
+            torch.cuda.synchronize()
+            res.append((weff[0], weff[1], dctxn, rowdot, dw_out))
         for i in range(4):
             assert torch.equal(res[0][i], res[1][i]), (B, dim, i)
         assert rel(res[1][4], res[0][4]) < 1e-5, (B, dim)
-    # attn_bwd_kv_kernel<REMAP>: one head and four pixel quads per warp; same sums in the same order
+        cn = ctx.double() / ksum.double().view(B, 4, 32, 1)
+        wo4, dwe = w_out.double().view(dim, 4, 32), dweff.double().view(B, dim, 4, 32)
+        want_weff = 0.17 * torch.einsum('ohe,bhde->bohd', wo4, cn).reshape(B, dim, 128)
+        want_dc = 0.17 * torch.einsum('bohd,ohe->bhde', dwe, wo4)
+        want_dw = 0.17 * torch.einsum('bohd,bhde->ohe', dwe, cn).reshape(dim, 128)
+        assert rel(res[0][0], want_weff) < 1e-5 and rel(res[0][1], want_weff) < 1e-3, (B, dim)
+        assert rel(res[0][2], want_dc) < 1e-5 and rel(res[0][3], (want_dc * cn).sum(-1).reshape(B, 128)) < 1e-5, (B, dim)
+        assert rel(res[0][4], want_dw) < 1e-5, (B, dim)
     for B, n in ((4, 4096), (2, 1000), (3, 40)):
-        qkv = torch.randn(B, n, 384, generator=gen).cuda()
-        kmax = qkv[:, :, 128:256].max(dim=1).values.contiguous()
-        ksum = torch.exp(qkv[:, :, 128:256] - kmax[:, None, :]).sum(dim=1).contiguous()
-        dctxn, rowdot = torch.randn(B, 4, 32, 32, generator=gen).cuda(), torch.randn(B, 128, generator=gen).cuda()
-        outs = []
-        try:
-            for staged in (0, 1):
-                lib.cd_linattn_set_staged(staged)
-                dqkv = torch.full((B, n, 384), 7.0, device='cuda')
-                _check(lib.cd_linattn_bwd_kv(ptr(qkv), 384, B, n, ptr(kmax), ptr(ksum), ptr(dctxn), ptr(rowdot), ptr(dqkv), 384, stream()), 'bwd_kv')
-                torch.cuda.synchronize()
-                outs.append(dqkv)
-        finally:
-            lib.cd_linattn_set_staged(0)
-        assert torch.equal(outs[0], outs[1]), (B, n)
-        # context_kernel<PRELOAD>: same values and partial sums; float atomics across blocks -> agreement to rounding
-        cres = []
-        try:
-            for staged in (0, 1):
-                lib.cd_linattn_set_staged(staged)
-                km, ks, cx = torch.empty(B, 128, device='cuda'), torch.empty(B, 128, device='cuda'), torch.empty(B, 4, 32, 32, device='cuda')
-                _check(lib.cd_linattn_context(ptr(qkv), 384, B, n, ptr(km), ptr(ks), ptr(cx), stream()), 'context')
-                torch.cuda.synchronize()
-                cres.append((km, ks, cx))
-        finally:
-            lib.cd_linattn_set_staged(0)
-        assert torch.equal(cres[0][0], cres[1][0]) and rel(cres[1][1], cres[0][1]) < 1e-5 and rel(cres[1][2], cres[0][2]) < 1e-5, (B, n)
+        for ld in (384, 385):
+            qkv = torch.randn(B, n, ld, generator=gen).cuda()
+            k, v = qkv[:, :, 128:256].double(), qkv[:, :, 256:384].double()
+            kmax = k.max(dim=1).values
+            e = torch.exp(k - kmax[:, None, :])
+            ksum = e.sum(dim=1)
+            want_ctx = torch.einsum('bnhd,bnhe->bhde', e.view(B, n, 4, 32), v.view(B, n, 4, 32))
+            dctxn, rowdot = torch.randn(B, 4, 32, 32, generator=gen).cuda(), torch.randn(B, 128, generator=gen).cuda()
+            dqkv = torch.full((B, n, 384), 7.0, device='cuda')
+            km32, ks32 = kmax.float().contiguous(), ksum.float().contiguous()
+            _check(lib.cd_linattn_bwd_kv(ptr(qkv), ld, B, n, ptr(km32), ptr(ks32), ptr(dctxn), ptr(rowdot), ptr(dqkv), 384, stream()), 'bwd_kv')
+            torch.cuda.synchronize()
+            Pm = (e / ksum[:, None, :]).view(B, n, 4, 32)
+            dc = dctxn.double()
+            want_dk = Pm * (torch.einsum('bhde,bnhe->bnhd', dc, v.view(B, n, 4, 32)) - rowdot.double().view(B, 1, 4, 32))
+            want_dv = torch.einsum('bnhd,bhde->bnhe', Pm, dc)
+            assert rel(dqkv[:, :, 128:256], want_dk.reshape(B, n, 128)) < 1e-5, (B, n, ld)
+            assert rel(dqkv[:, :, 256:384], want_dv.reshape(B, n, 128)) < 1e-5, (B, n, ld)
+            assert bool((dqkv[:, :, :128] == 7.0).all()), (B, n, ld)
+            if ld % 4:
+                continue
+            ppb = 64
+            nblk = -(-n // ppb)
+            ws = torch.empty(B, nblk, 4352, device='cuda')
+            km, ks, cx = torch.empty(B, 128, device='cuda'), torch.empty(B, 128, device='cuda'), torch.empty(B, 4, 32, 32, device='cuda')
+            _check(lib.cd_linattn_context_det(ptr(qkv), ld, B, n, nblk, ppb, ptr(ws), ptr(km), ptr(ks), ptr(cx), stream()), 'context_det')
+            torch.cuda.synchronize()
+            assert torch.equal(km, kmax.float()), (B, n)
+            assert rel(ks, ksum) < 1e-5 and rel(cx, want_ctx) < 1e-5, (B, n)
 
 
-@OPT_IN
-def test_layernorm_multi_pixel_forward_matches_the_default_kernel():
-    """csrc/layernorm_multi.cu (cd_layernorm_set_multi): same per-pixel
-    arithmetic as layernorm_kernel<1> -> bit-identical output and statistics"""
+def test_layernorm_multi_pixel_forward_against_float64():
+    """csrc/layernorm_multi.cu (4 pixels per lane group in flight on 4096 pixels or more): the same per-pixel arithmetic as
+    layernorm_kernel<1>, which serves fewer pixels (here the same rows in slices of 4095 pixels) -> bit-identical output and
+    statistics; statistics and output against float64"""
     import ctypes as C
     from cold_diffusion_models_b200._lib import lib, ptr, stream, _check
     gen = torch.Generator().manual_seed(4)
@@ -314,26 +328,30 @@ def test_layernorm_multi_pixel_forward_matches_the_default_kernel():
         x = (torch.randn(npix, ld, generator=gen) * 3 + 0.5).cuda()
         gam, bet = (1 + 0.2 * torch.randn(Cc, generator=gen)).cuda(), (0.1 * torch.randn(Cc, generator=gen)).cuda()
         res = []
-        try:
-            for pp in (0, 2, 4):
-                lib.cd_layernorm_set_multi(pp)
-                y, st = torch.full((npix, ld), 7.0, device='cuda'), torch.full((npix, 2), 7.0, device='cuda')
-                _check(lib.cd_layernorm_fwd(ptr(x), ld, C.c_int64(npix), Cc, ptr(gam), ptr(bet), C.c_float(1e-5), ptr(y), ld, ptr(st), 1, stream()), 'ln')
-                torch.cuda.synchronize()
-                res.append((y, st))
-        finally:
-            lib.cd_layernorm_set_multi(0)
-        for y, st in res[1:]:
-            assert torch.equal(y, res[0][0]) and torch.equal(st, res[0][1]), (npix, Cc)
+        for sl in (npix, 4095):
+            y, st = torch.full((npix, ld), 7.0, device='cuda'), torch.full((npix, 2), 7.0, device='cuda')
+            for p0 in range(0, npix, sl):
+                m = min(sl, npix - p0)
+                _check(lib.cd_layernorm_fwd(ptr(x[p0:]), ld, C.c_int64(m), Cc, ptr(gam), ptr(bet), C.c_float(1e-5), ptr(y[p0:]), ld,
+                                            ptr(st[p0:]), 1, stream()), 'ln')
+            torch.cuda.synchronize()
+            res.append((y, st))
+        assert torch.equal(res[0][0], res[1][0]) and torch.equal(res[0][1], res[1][1]), (npix, Cc)
+        xm = x[:, :Cc].double()
+        mean, var = xm.mean(1), xm.var(1, unbiased=False)
+        want = (xm - mean[:, None]) / torch.sqrt(var[:, None] + 1e-5) * gam.double() + bet.double()
+        assert rel(res[0][1][:, 0], mean) < 1e-5 and rel(res[0][1][:, 1], 1 / torch.sqrt(var + 1e-5)) < 1e-5, (npix, Cc)
+        assert rel(res[0][0][:, :Cc], want) < 1e-3 and bool((res[0][0][:, Cc:] == 7.0).all()), (npix, Cc)
 
 
-@OPT_IN
-def test_image_edge_kernels_with_preloaded_staging_match_the_default():
-    """cd_conv_simt_set_preload: the 3-channel image-edge convolution and its
-    weight gradient with all receptive-field loads of a chunk in flight; outputs bit-identical, weight gradients (float atomics over
-    blocks) to rounding"""
+def test_image_edge_kernels_against_float64():
+    """the 3-channel image-edge convolution and its weight gradient (register-tiled kernels with all receptive-field loads of a
+    chunk in flight), the final 1x1 projection NHWC -> NCHW through a shared-memory tile (csrc/final_proj.cu), its backward with
+    four pixels per trip and the float4 batched column sums, all against float64"""
+    import ctypes as C
+    import torch.nn.functional as F
     from cold_diffusion_models_b200 import ops
-    from cold_diffusion_models_b200._lib import lib
+    from cold_diffusion_models_b200._lib import lib, ptr, stream, _check
     gen = torch.Generator().manual_seed(8)
     for Cout, k, B, H in ((128, 3, 8, 128), (64, 1, 8, 128), (128, 3, 3, 32)):
         x = torch.zeros(B, H, H, 4)
@@ -342,67 +360,42 @@ def test_image_edge_kernels_with_preloaded_staging_match_the_default():
         taps = ops.taps_conv(k, k // 2)
         wp, bias = (torch.randn(len(taps), Cout, 3, generator=gen) / 3).cuda(), torch.randn(Cout, generator=gen).cuda()
         dy = torch.randn(B, H, H, Cout, generator=gen).cuda()
-        res = []
-        try:
-            for pre in (0, 1):
-                lib.cd_conv_simt_set_preload(pre)
-                out, pa = torch.full((B, H, H, Cout), 7.0, device='cuda'), torch.full((B, H, H, Cout), 7.0, device='cuda')
-                d = ops.make_conv_desc([(ops.View(x, 0, 3), taps, wp, False)], ops.View(out), (B, H, H), Cout=Cout, bias=bias, act=ops.ACT_GELU,
-                                       out2=ops.View(pa))
-                ops.conv_fwd(d, ops.CONV_SIMT)
-                dw, db = torch.zeros(len(taps), Cout, 3, device='cuda'), torch.zeros(Cout, device='cuda')
-                dd = ops.make_conv_desc([(ops.View(x, 0, 3), taps, dw, False)], ops.View(dy), (B, H, H), Cout=Cout)
-                ops.conv_wgrad(dd, ops.View(dy), dw, db, impl=ops.CONV_SIMT)
-                torch.cuda.synchronize()
-                res.append((out, pa, dw, db))
-        finally:
-            lib.cd_conv_simt_set_preload(0)
-        assert torch.equal(res[0][0], res[1][0]) and torch.equal(res[0][1], res[1][1]), (Cout, k)
-        assert rel(res[1][2], res[0][2]) < 1e-5 and rel(res[1][3], res[0][3]) < 1e-5, (Cout, k)
-    # the same switch: final 1x1 projection NHWC -> NCHW through a shared-memory tile (csrc/final_proj.cu), bit-identical
-    import ctypes as C
-    from cold_diffusion_models_b200._lib import ptr, stream, _check
+        out, pa = torch.full((B, H, H, Cout), 7.0, device='cuda'), torch.full((B, H, H, Cout), 7.0, device='cuda')
+        d = ops.make_conv_desc([(ops.View(x, 0, 3), taps, wp, False)], ops.View(out), (B, H, H), Cout=Cout, bias=bias, act=ops.ACT_GELU,
+                               out2=ops.View(pa))
+        ops.conv_fwd(d, ops.CONV_SIMT)
+        dw, db = torch.zeros(len(taps), Cout, 3, device='cuda'), torch.zeros(Cout, device='cuda')
+        dd = ops.make_conv_desc([(ops.View(x, 0, 3), taps, dw, False)], ops.View(dy), (B, H, H), Cout=Cout)
+        ops.conv_wgrad(dd, ops.View(dy), dw, db, impl=ops.CONV_SIMT)
+        torch.cuda.synchronize()
+        x64 = x[..., :3].double().permute(0, 3, 1, 2)
+        w64 = wp.double().view(k, k, Cout, 3).permute(2, 3, 0, 1).contiguous().requires_grad_(True)
+        ref = F.conv2d(x64, w64, bias.double(), padding=k // 2)
+        (ref * dy.double().permute(0, 3, 1, 2)).sum().backward()
+        assert rel(pa, ref.detach().permute(0, 2, 3, 1)) < 1e-5 and rel(out, F.gelu(ref.detach()).permute(0, 2, 3, 1)) < 1e-5, (Cout, k)
+        assert rel(dw, w64.grad.permute(2, 3, 0, 1).reshape(len(taps), Cout, 3)) < 1e-5, (Cout, k)
+        assert rel(db, dy.double().sum(dim=(0, 1, 2))) < 1e-5, (Cout, k)
     for B, H, Cc, Co in ((32, 128, 64, 3), (3, 17, 64, 3), (2, 16, 32, 1)):
         x = torch.randn(B, H, H, Cc, generator=gen).cuda()
         w, bias = (torch.randn(Co, Cc, generator=gen) / 8).cuda(), torch.randn(Co, generator=gen).cuda()
         r = torch.randn(B, Co, H, H, generator=gen).cuda()
-        outs = []
-        try:
-            for pre in (0, 1):
-                lib.cd_conv_simt_set_preload(pre)
-                o = torch.full((B, Co, H, H), 7.0, device='cuda')
-                _check(lib.cd_conv1x1_to_nchw(ptr(x), Cc, B, H, H, Cc, ptr(w), ptr(bias), Co, ptr(r), ptr(o), stream()), 'final projection')
-                torch.cuda.synchronize()
-                outs.append(o)
-        finally:
-            lib.cd_conv_simt_set_preload(0)
-        assert torch.equal(outs[0], outs[1]), (B, H, Cc, Co)
-        # ... and its backward with four pixels per trip in flight: same order of every sum per thread; dW / db go through float atomics
-        bres = []
-        try:
-            for pre in (0, 1):
-                lib.cd_conv_simt_set_preload(pre)
-                dx, dw, db = torch.full((B, H, H, Cc), 7.0, device='cuda'), torch.zeros(Co, Cc, device='cuda'), torch.zeros(Co, device='cuda')
-                _check(lib.cd_conv1x1_to_nchw_bwd(ptr(r), ptr(x), Cc, B, H, H, Cc, ptr(w), Co, ptr(dx), Cc, ptr(dw), ptr(db), stream()), 'final projection bwd')
-                torch.cuda.synchronize()
-                bres.append((dx, dw, db))
-        finally:
-            lib.cd_conv_simt_set_preload(0)
-        assert torch.equal(bres[0][0], bres[1][0]) and rel(bres[1][1], bres[0][1]) < 1e-5 and rel(bres[1][2], bres[0][2]) < 1e-5, (B, H, Cc, Co)
-    # ... and the float4 variant of the batched column sums (time-conditioning gradient): another summation order, fp32 rounding
+        o = torch.full((B, Co, H, H), 7.0, device='cuda')
+        _check(lib.cd_conv1x1_to_nchw(ptr(x), Cc, B, H, H, Cc, ptr(w), ptr(bias), Co, ptr(r), ptr(o), stream()), 'final projection')
+        torch.cuda.synchronize()
+        want = torch.einsum('bhwc,oc->bohw', x.double(), w.double()) + bias.double()[None, :, None, None] + r.double()
+        assert rel(o, want) < 1e-5, (B, H, Cc, Co)
+        dx, dw, db = torch.full((B, H, H, Cc), 7.0, device='cuda'), torch.zeros(Co, Cc, device='cuda'), torch.zeros(Co, device='cuda')
+        _check(lib.cd_conv1x1_to_nchw_bwd(ptr(r), ptr(x), Cc, B, H, H, Cc, ptr(w), Co, ptr(dx), Cc, ptr(dw), ptr(db), stream()), 'final projection bwd')
+        torch.cuda.synchronize()
+        assert rel(dx, torch.einsum('bohw,oc->bhwc', r.double(), w.double())) < 1e-5, (B, H, Cc, Co)
+        assert rel(dw, torch.einsum('bohw,bhwc->oc', r.double(), x.double())) < 1e-5, (B, H, Cc, Co)
+        assert rel(db, r.double().sum(dim=(0, 2, 3))) < 1e-5, (B, H, Cc, Co)
     for B, rows, Cc in ((32, 16384, 64), (3, 300, 128), (2, 256, 512)):
         x = torch.randn(B, rows, Cc, generator=gen).cuda()
-        cres = []
-        try:
-            for pre in (0, 1):
-                lib.cd_conv_simt_set_preload(pre)
-                o = torch.full((B, Cc + 16), 0.5, device='cuda')
-                _check(lib.cd_colsum_batched(ptr(x), Cc, B, C.c_int64(rows), Cc, ptr(o), Cc + 16, stream()), 'colsum_batched')
-                torch.cuda.synchronize()
-                cres.append(o)
-        finally:
-            lib.cd_conv_simt_set_preload(0)
-        assert rel(cres[1], cres[0]) < 1e-5 and bool((cres[1][:, Cc:] == 0.5).all()), (B, rows, Cc)
+        o = torch.full((B, Cc + 16), 0.5, device='cuda')
+        _check(lib.cd_colsum_batched(ptr(x), Cc, B, C.c_int64(rows), Cc, ptr(o), Cc + 16, stream()), 'colsum_batched')
+        torch.cuda.synchronize()
+        assert rel(o[:, :Cc], 0.5 + x.double().sum(dim=1)) < 1e-5 and bool((o[:, Cc:] == 0.5).all()), (B, rows, Cc)
 
 
 @OPT_IN

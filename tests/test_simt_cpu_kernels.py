@@ -1,4 +1,4 @@
-"""The CUDA SOURCE of SIMT kernels that are off by default, executed on the CPU (tests/simt_cpu: the .cu file is compiled
+"""The CUDA SOURCE of SIMT kernels, executed on the CPU (tests/simt_cpu: the .cu file is compiled
 by g++ against a shim <cuda_runtime.h>, every CUDA thread is a fiber, barriers and warp shuffles are scheduling points) and
 compared with the numpy statement of the same entry point in tests/abi_emulator.py, which in turn is pinned to the reference
 goldens by tests/test_model2_host_logic.py.  Catches indexing, reduction and launch-geometry mistakes in the kernels themselves;
@@ -192,65 +192,76 @@ def test_time_mlp2_source_both_paths(cpulib, with_temb, B, dim, hid, tdim, act, 
         assert close(got, want, 2e-4)            # sin / cos of arguments up to 999 in fp32, then three dense layers
 
 
+def unaligned(t):
+    """a copy of `t` whose data starts 4 bytes past a 16-byte boundary (selects the kernels that take any alignment)"""
+    buf = torch.empty(t.numel() + 1, dtype=t.dtype)
+    u = buf[1:].view(t.shape)
+    u.copy_(t)
+    assert u.data_ptr() % 16 != 0
+    return u
+
+
 @pytest.mark.parametrize('B,dim', [(2, 64), (3, 512), (1, 40), (2, 100)])
-def test_linattn_staged_kernels_equal_the_default_ones(cpulib, B, dim):
-    """csrc/linattn_small.cu (cd_linattn_set_staged): the shared-memory-staged cd_linattn_weff / cd_linattn_bwd_small keep the
-    arithmetic order of the default kernels -> bit-identical results (the CPU execution runs the blocks, hence the float atomics
-    into dW_out, in the same order for both); both also agree with the numpy statement"""
+def test_linattn_staged_kernels_equal_the_unaligned_fallback(cpulib, B, dim):
+    """csrc/linattn_small.cu: the shared-memory-staged cd_linattn_weff / cd_linattn_bwd_small keep the arithmetic order of
+    weff_kernel / attn_bwd_small_kernel, which serve a w_out / dweff that is not 16-byte aligned -> bit-identical results (the CPU
+    execution runs the blocks, hence the float atomics into dW_out, in the same order for both); every output also agrees with
+    the float64 numpy statement"""
     g = torch.Generator().manual_seed(B * 7 + dim)
     r = lambda *s: torch.randn(*s, generator=g)
     ctx, ksum, w_out, dweff = r(B, 4, 32, 32), 1.0 + torch.rand(B, 128, generator=g) * 30, r(dim, 128) / 11, r(B, dim, 128)
     res = {}
     for order in (0, 1):
         cpulib.simt_set_reverse_order(order)
-        for staged in (0, 1):
-            assert cpulib.cd_linattn_set_staged(staged) == 0
+        for aligned in (1, 0):
+            wo, dwe = (w_out, dweff) if aligned else (unaligned(w_out), unaligned(dweff))
             for rnd in (0, 1):
                 weff = torch.full((B, dim, 128), 7.0)
-                assert cpulib.cd_linattn_weff(P(ctx), P(ksum), P(w_out), B, dim, C.c_float(0.17), rnd, P(weff), C.c_void_p(0)) == 0
-                res[('weff', rnd, staged, order)] = weff
+                assert cpulib.cd_linattn_weff(P(ctx), P(ksum), P(wo), B, dim, C.c_float(0.17), rnd, P(weff), C.c_void_p(0)) == 0
+                res[('weff', rnd, aligned, order)] = weff
             dw_out, dctxn, rowdot = 0.5 * torch.ones(dim, 128), torch.full((B, 4, 32, 32), 7.0), torch.full((B, 128), 7.0)
-            assert cpulib.cd_linattn_bwd_small(P(dweff), P(ctx), P(ksum), P(w_out), B, dim, C.c_float(0.17), P(dw_out), P(dctxn), P(rowdot),
+            assert cpulib.cd_linattn_bwd_small(P(dwe), P(ctx), P(ksum), P(w_out), B, dim, C.c_float(0.17), P(dw_out), P(dctxn), P(rowdot),
                                                C.c_void_p(0)) == 0
-            res[('bwd', 0, staged, order)] = torch.cat([dw_out.reshape(-1), dctxn.reshape(-1), rowdot.reshape(-1)])
-    cpulib.cd_linattn_set_staged(0)
+            res[('bwd', 0, aligned, order)] = torch.cat([dw_out.reshape(-1), dctxn.reshape(-1), rowdot.reshape(-1)])
     cpulib.simt_set_reverse_order(0)
     for key in [('weff', 0), ('weff', 1), ('bwd', 0)]:
         base = res[key + (0, 0)]
-        for staged in (0, 1):
+        for aligned in (0, 1):
             for order in (0, 1):
-                assert torch.equal(res[key + (staged, order)], base), (key, staged, order)
+                assert torch.equal(res[key + (aligned, order)], base), (key, aligned, order)
     weff = torch.zeros(B, dim, 128)
     assert E.cd_linattn_weff(P(ctx), P(ksum), P(w_out), B, dim, C.c_float(0.17), 0, P(weff), None) == 0
     assert close(res[('weff', 0, 1, 0)], weff, 1e-5)
     dw_out, dctxn, rowdot = 0.5 * torch.ones(dim, 128), torch.zeros(B, 4, 32, 32), torch.zeros(B, 128)
     assert E.cd_linattn_bwd_small(P(dweff), P(ctx), P(ksum), P(w_out), B, dim, C.c_float(0.17), P(dw_out), P(dctxn), P(rowdot), None) == 0
-    assert close(res[('bwd', 0, 1, 0)], torch.cat([dw_out.reshape(-1), dctxn.reshape(-1), rowdot.reshape(-1)]), 1e-4)
+    got = res[('bwd', 0, 1, 0)]
+    assert close(got, torch.cat([dw_out.reshape(-1), dctxn.reshape(-1), rowdot.reshape(-1)]), 1e-4)
+    n0, n1 = dim * 128, dim * 128 + B * 4096
+    assert close(got[:n0], dw_out.reshape(-1), 1e-4)
+    assert close(got[n0:n1], dctxn.reshape(-1), 1e-4)
+    assert close(got[n1:], rowdot.reshape(-1), 1e-4)
 
 
-@pytest.mark.parametrize('B,n,ld,dld', [(2, 256, 384, 384), (1, 1000, 392, 388), (3, 40, 384, 384)])
-def test_linattn_bwd_kv_remapped_equals_the_default_mapping(cpulib, B, n, ld, dld):
-    """attn_bwd_kv_kernel<REMAP> (cd_linattn_set_staged): a warp owns one head and four pixel quads instead of four heads and one
-    pixel quad (4x fewer shared-memory wavefronts); the same sums in the same order -> bit-identical, also for a ragged last tile"""
+@pytest.mark.parametrize('B,n,ld,dld,misalign', [(2, 256, 385, 384, False), (1, 1000, 393, 388, False), (3, 40, 387, 384, False),
+                                                 (2, 256, 384, 384, True)])
+def test_linattn_bwd_kv_cuda_core_kernel(cpulib, B, n, ld, dld, misalign):
+    """attn_bwd_kv_kernel (csrc/backward.cu), which serves the qkv the tensor-core kernel refuses (ld % 4 != 0, or qkv not 16-byte
+    aligned): a warp owns one head and four pixel quads; identical under both thread orders, also for a ragged last tile, and
+    dk / dv at fp32 accuracy against the float64 statement; q columns and row padding untouched"""
     g = torch.Generator().manual_seed(n)
     qkv = torch.randn(B, n, ld, generator=g)
     kmax = qkv[:, :, 128:256].max(dim=1).values.contiguous()
     ksum = torch.exp(qkv[:, :, 128:256] - kmax[:, None, :]).sum(dim=1).contiguous()
     dctxn, rowdot = torch.randn(B, 4, 32, 32, generator=g), torch.randn(B, 128, generator=g)
+    q_in = unaligned(qkv) if misalign else qkv
     res = []
-    cpulib.cd_linattn_set_bwd_mma(0)                 # the CUDA-core kernels (the tensor-core one is the default: next test)
     for order in (0, 1):
         cpulib.simt_set_reverse_order(order)
-        for staged in (0, 1):
-            cpulib.cd_linattn_set_staged(staged)
-            dqkv = torch.full((B, n, dld), 7.0)
-            assert cpulib.cd_linattn_bwd_kv(P(qkv), ld, B, n, P(kmax), P(ksum), P(dctxn), P(rowdot), P(dqkv), dld, C.c_void_p(0)) == 0
-            res.append(dqkv)
-    cpulib.cd_linattn_set_staged(0)
-    cpulib.cd_linattn_set_bwd_mma(1)
+        dqkv = torch.full((B, n, dld), 7.0)
+        assert cpulib.cd_linattn_bwd_kv(P(q_in), ld, B, n, P(kmax), P(ksum), P(dctxn), P(rowdot), P(dqkv), dld, C.c_void_p(0)) == 0
+        res.append(dqkv)
     cpulib.simt_set_reverse_order(0)
-    for r in res[1:]:
-        assert torch.equal(r, res[0])
+    assert torch.equal(res[0], res[1])
     want = torch.full((B, n, dld), 7.0)
     assert E.cd_linattn_bwd_kv(P(qkv), ld, B, n, P(kmax), P(ksum), P(dctxn), P(rowdot), P(want), dld, None) == 0
     assert close(res[1][:, :, 128:384], want[:, :, 128:384], 2e-5)
@@ -259,7 +270,7 @@ def test_linattn_bwd_kv_remapped_equals_the_default_mapping(cpulib, B, n, ld, dl
 
 @pytest.mark.parametrize('B,n,ld,dld', [(2, 256, 384, 384), (1, 1000, 392, 388), (3, 40, 384, 384), (1, 16, 384, 384)])
 def test_linattn_bwd_kv_tensor_core_kernel(cpulib, B, n, ld, dld):
-    """attn_bwd_kv_mma_kernel (csrc/linattn_bwd.cu, the default behind cd_linattn_bwd_kv): mma.sync fragments in the 3xTF32 split
+    """attn_bwd_kv_mma_kernel (csrc/linattn_bwd.cu, what cd_linattn_bwd_kv runs on aligned operands): mma.sync fragments in the 3xTF32 split
     -> dk / dv at fp32 accuracy against the float64 statement; ragged spans; q columns and row padding untouched; identical
     under both thread orders"""
     g = torch.Generator().manual_seed(n + 1)
@@ -282,9 +293,10 @@ def test_linattn_bwd_kv_tensor_core_kernel(cpulib, B, n, ld, dld):
 
 
 @pytest.mark.parametrize('npix,C,pad,stats,rnd', [(4096, 64, 0, True, 1), (5000, 128, 8, False, 0), (4099, 32, 4, True, 0), (70000, 64, 0, True, 0)])
-def test_layernorm_multi_pixel_forward_equals_the_default_kernel(cpulib, npix, C, pad, stats, rnd):
-    """csrc/layernorm_multi.cu (cd_layernorm_set_multi): 2 / 4 pixels per lane group in flight, same per-pixel arithmetic ->
-    bit-identical to layernorm_kernel<1>, ragged pixel counts and padded rows included"""
+def test_layernorm_multi_pixel_forward_equals_the_fallback_kernel(cpulib, npix, C, pad, stats, rnd):
+    """csrc/layernorm_multi.cu: 4 pixels per lane group in flight on 4096 pixels or more, same per-pixel arithmetic ->
+    bit-identical to layernorm_kernel<1>, which serves fewer pixels (here the same rows in slices of 4095 pixels); ragged pixel
+    counts and padded rows included; identical under both thread orders; output against the float64 statement"""
     g = torch.Generator().manual_seed(npix + C)
     ld = C + pad
     x = torch.randn(npix, ld, generator=g) * 3 + 0.5
@@ -292,13 +304,13 @@ def test_layernorm_multi_pixel_forward_equals_the_default_kernel(cpulib, npix, C
     res = []
     for order in (0, 1):
         cpulib.simt_set_reverse_order(order)
-        for pp in (0, 2, 4):
-            cpulib.cd_layernorm_set_multi(pp)
+        for sl in (npix, 4095):
             y, st = torch.full((npix, ld), 7.0), (torch.full((npix, 2), 7.0) if stats else None)
-            assert cpulib.cd_layernorm_fwd(P(x), ld, ctypes_mod.c_int64(npix), C, P(gam), P(bet),
-                                           ctypes_mod.c_float(1e-5), P(y), ld, P(st), rnd, None) == 0
+            for p0 in range(0, npix, sl):
+                m = min(sl, npix - p0)
+                assert cpulib.cd_layernorm_fwd(P(x[p0:]), ld, ctypes_mod.c_int64(m), C, P(gam), P(bet), ctypes_mod.c_float(1e-5),
+                                               P(y[p0:]), ld, P(st[p0:] if stats else None), rnd, None) == 0
             res.append((y, st))
-    cpulib.cd_layernorm_set_multi(0)
     cpulib.simt_set_reverse_order(0)
     for y, st in res[1:]:
         assert torch.equal(y, res[0][0])
@@ -307,30 +319,10 @@ def test_layernorm_multi_pixel_forward_equals_the_default_kernel(cpulib, npix, C
     assert bool((res[0][0][:, C:] == 7.0).all())
     xm = x[:, :C].double()
     want = (xm - xm.mean(1, keepdim=True)) / torch.sqrt(xm.var(1, unbiased=False, keepdim=True) + 1e-5) * gam.double() + bet.double()
-    assert close(res[2][0][:, :C], want.float(), 2e-3 if rnd else 2e-5)
-
-
-@pytest.mark.parametrize('B,n,ld', [(2, 256, 384), (1, 1000, 392), (3, 40, 384)])
-def test_linattn_context_preload_variant_equals_the_default(cpulib, B, n, ld):
-    """context_kernel<PRELOAD> (cd_linattn_set_staged): all loads of a chunk requested before the first use; the same values and
-    the same order of partial sums -> kmax / ksum / ctx bit-identical on the CPU executor (deterministic block order)"""
-    g = torch.Generator().manual_seed(n + ld)
-    qkv = torch.randn(B, n, ld, generator=g)
-    res = []
-    for order in (0, 1):
-        cpulib.simt_set_reverse_order(order)
-        for staged in (0, 1):
-            cpulib.cd_linattn_set_staged(staged)
-            kmax, ksum, ctx = torch.full((B, 128), 7.0), torch.full((B, 128), 7.0), torch.full((B, 4, 32, 32), 7.0)
-            assert cpulib.cd_linattn_context(P(qkv), ld, B, n, P(kmax), P(ksum), P(ctx), C.c_void_p(0)) == 0
-            res.append(torch.cat([kmax.reshape(-1), ksum.reshape(-1), ctx.reshape(-1)]))
-    cpulib.cd_linattn_set_staged(0)
-    cpulib.simt_set_reverse_order(0)
-    assert torch.equal(res[0], res[1]) and torch.equal(res[2], res[3])          # per thread order: staged == default
-    assert close(res[1], res[3], 1e-5)                                           # across thread orders the float atomics reorder
-    kmax, ksum, ctx = torch.zeros(B, 128), torch.zeros(B, 128), torch.zeros(B, 4, 32, 32)
-    assert E.cd_linattn_context(P(qkv), ld, B, n, P(kmax), P(ksum), P(ctx), None) == 0
-    assert close(res[1], torch.cat([kmax.reshape(-1), ksum.reshape(-1), ctx.reshape(-1)]), 2e-5)
+    assert close(res[0][0][:, :C], want.float(), 2e-3 if rnd else 2e-5)
+    if stats:
+        assert close(res[0][1][:, 0], xm.mean(1).float(), 2e-5)
+        assert close(res[0][1][:, 1], (1 / torch.sqrt(xm.var(1, unbiased=False) + 1e-5)).float(), 2e-5)
 
 
 @pytest.mark.parametrize('B,n,ld,ppb', [(2, 256, 384, 64), (1, 1000, 392, 96), (3, 40, 384, 64), (1, 16, 384, 64)])
@@ -356,44 +348,58 @@ def test_linattn_context_deterministic_one_pass_kernel(cpulib, B, n, ld, ppb):
     assert close(res[0], torch.cat([kmax.reshape(-1), ksum.reshape(-1), ctx.reshape(-1)]), 3e-6)
 
 
-@pytest.mark.parametrize('Cout,k', [(128, 3), (64, 1)])
-def test_image_edge_kernels_with_preloaded_staging_equal_the_default(cpulib, Cout, k):
-    """cd_conv_simt_set_preload: conv_smallc4_kernel / wgrad_smallc4_kernel (3-channel image edge) with all receptive-field
-    entries of a chunk loaded before the first store -> bit-identical outputs and weight gradients"""
+def conv_taps_f64(x, taps, w):
+    """float64 tap-list convolution: out[b, y, x, o] = sum_t sum_c x[b, y + dy_t, x + dx_t, c] w[t, o, c], zero outside the image"""
+    B, H, W, _ = x.shape
+    pad = 4
+    xp = torch.nn.functional.pad(x.double(), (0, 0, pad, pad, pad, pad))
+    return sum(torch.einsum('bhwc,oc->bhwo', xp[:, pad + tp[2]:pad + tp[2] + H, pad + tp[3]:pad + tp[3] + W], w[t].double())
+               for t, tp in enumerate(taps))
+
+
+@pytest.mark.parametrize('Cout,k,Cin', [(128, 3, 3), (64, 1, 3), (64, 4, 2)])
+def test_image_edge_kernels_against_float64(cpulib, Cout, k, Cin):
+    """conv_smallc4_kernel / wgrad_smallc4_kernel (image edge, Cin <= 4): receptive fields staged with all loads of a chunk in
+    flight (stage_patches_preload) for up to 12 taps, by the plain loop (stage_patches) for the 16 taps of a 4 x 4 kernel;
+    outputs and pre-activations identical under both thread orders; those and the weight / bias gradients (float atomics) at
+    fp32 accuracy against float64"""
     from cold_diffusion_models_b200 import ops
     g = torch.Generator().manual_seed(Cout + k)
     B, H = 2, 24                                            # 1152 pixels: 18 chunks of 64
     x = torch.zeros(B, H, H, 4)
-    x[..., :3] = torch.randn(B, H, H, 3, generator=g)
-    taps = ops.taps_conv(k, k // 2)
-    wp = torch.randn(len(taps), Cout, 3, generator=g) / 3
+    x[..., :Cin] = torch.randn(B, H, H, Cin, generator=g)
+    taps = ops.taps_conv(k, (k - 1) // 2)
+    wp = torch.randn(len(taps), Cout, Cin, generator=g) / 3
     bias, dy = torch.randn(Cout, generator=g), torch.randn(B, H, H, Cout, generator=g)
     res = []
     for order in (0, 1):
         cpulib.simt_set_reverse_order(order)
-        for pre in (0, 1):
-            cpulib.cd_conv_simt_set_preload(pre)
-            out, pre_act = torch.full((B, H, H, Cout), 7.0), torch.full((B, H, H, Cout), 7.0)
-            d = ops.make_conv_desc([(ops.View(x, 0, 3), taps, wp, False)], ops.View(out), (B, H, H), Cout=Cout, bias=bias, act=ops.ACT_GELU,
-                                   out2=ops.View(pre_act))
-            assert cpulib.cd_conv_fwd(C.byref(d), 0, None) == 0
-            dw, db = torch.zeros(len(taps), Cout, 3), torch.zeros(Cout)
-            dd = ops.make_conv_desc([(ops.View(x, 0, 3), taps, dw, False)], ops.View(dy), (B, H, H), Cout=Cout)
-            assert cpulib.cd_conv_wgrad(C.byref(dd), P(dy), Cout, P(dw), P(db), 0, None) == 0
-            res.append((out, pre_act, dw, db))
-    cpulib.cd_conv_simt_set_preload(0)
+        out, pre_act = torch.full((B, H, H, Cout), 7.0), torch.full((B, H, H, Cout), 7.0)
+        d = ops.make_conv_desc([(ops.View(x, 0, Cin), taps, wp, False)], ops.View(out), (B, H, H), Cout=Cout, bias=bias, act=ops.ACT_GELU,
+                               out2=ops.View(pre_act))
+        assert cpulib.cd_conv_fwd(C.byref(d), 0, None) == 0
+        dw, db = torch.zeros(len(taps), Cout, Cin), torch.zeros(Cout)
+        dd = ops.make_conv_desc([(ops.View(x, 0, Cin), taps, dw, False)], ops.View(dy), (B, H, H), Cout=Cout)
+        assert cpulib.cd_conv_wgrad(C.byref(dd), P(dy), Cout, P(dw), P(db), 0, None) == 0
+        res.append((out, pre_act, dw, db))
     cpulib.simt_set_reverse_order(0)
-    for i in (0, 2):                                        # same thread order: preload == default, bit for bit
-        for a, b in zip(res[i], res[i + 1]):
-            assert torch.equal(a, b)
-    want = torch.einsum('bhwtc,toc->bhwo', torch.stack([torch.roll(torch.nn.functional.pad(x[..., :3], (0, 0, 1, 1, 1, 1)), (-tp[2], -tp[3]), (1, 2))[:, 1:-1, 1:-1] if k == 3 else x[..., :3] for tp in taps], dim=3), wp) + bias
-    assert close(res[1][1], want, 2e-5)
+    for a, b in zip(res[0][:2], res[1][:2]):                # forward: the same sums in the same order under both thread orders
+        assert torch.equal(a, b)
+    want = conv_taps_f64(x[..., :Cin], taps, wp) + bias.double()
+    assert close(res[1][1], want.float(), 2e-5)
+    assert close(res[1][0], torch.nn.functional.gelu(want).float(), 2e-5)
+    xs = x[..., :Cin].double()
+    want_dw = torch.stack([torch.einsum('bhwo,bhwc->oc', dy.double(), conv_taps_f64(xs, [tp], torch.eye(Cin)[None])) for tp in taps])
+    assert close(res[1][2], want_dw.float(), 2e-5)
+    assert close(res[1][3], dy.double().sum(dim=(0, 1, 2)).float(), 2e-5)
 
 
-@pytest.mark.parametrize('B,H,Cc,pad,Co,resid', [(2, 24, 64, 0, 3, True), (1, 17, 64, 8, 3, False), (3, 8, 32, 0, 1, True), (1, 16, 128, 0, 5, False)])
-def test_tiled_final_projection_equals_the_default_kernel(cpulib, B, H, Cc, pad, Co, resid):
-    """csrc/final_proj.cu (behind cd_conv_simt_set_preload): the NHWC -> NCHW 1x1 projection through a shared-memory tile, same order
-    of the dot products -> bit-identical, ragged last tile and padded rows included"""
+@pytest.mark.parametrize('B,H,Cc,pad,Co,resid', [(2, 24, 64, 0, 3, True), (1, 17, 64, 8, 3, False), (3, 8, 32, 0, 1, True), (1, 16, 128, 0, 5, False),
+                                                 (2, 12, 48, 0, 3, True)])
+def test_final_projection_tiled_and_fallback_against_float64(cpulib, B, H, Cc, pad, Co, resid):
+    """csrc/final_proj.cu: the NHWC -> NCHW 1x1 projection through a shared-memory tile (C = 32, 64, 128) and
+    conv1x1_to_nchw_kernel for the other C (here 48): identical under both thread orders and against the float64 statement,
+    ragged last tile and padded rows included"""
     g = torch.Generator().manual_seed(B * H + Cc)
     ld = Cc + pad
     x = torch.randn(B, H, H, ld, generator=g)
@@ -402,59 +408,51 @@ def test_tiled_final_projection_equals_the_default_kernel(cpulib, B, H, Cc, pad,
     res = []
     for order in (0, 1):
         cpulib.simt_set_reverse_order(order)
-        for pre in (0, 1):
-            cpulib.cd_conv_simt_set_preload(pre)
-            out = torch.full((B, Co, H, H), 7.0)
-            assert cpulib.cd_conv1x1_to_nchw(P(x), ld, B, H, H, Cc, P(w), P(bias), Co, P(r), P(out), None) == 0
-            res.append(out)
-    cpulib.cd_conv_simt_set_preload(0)
+        out = torch.full((B, Co, H, H), 7.0)
+        assert cpulib.cd_conv1x1_to_nchw(P(x), ld, B, H, H, Cc, P(w), P(bias), Co, P(r), P(out), None) == 0
+        res.append(out)
     cpulib.simt_set_reverse_order(0)
     for o in res[1:]:
         assert torch.equal(o, res[0])
     want = torch.einsum('bhwc,oc->bohw', x[..., :Cc].double(), w.double()) + bias.double()[None, :, None, None] + (r.double() if resid else 0)
-    assert close(res[1], want.float(), 2e-5)
+    assert close(res[0], want.float(), 2e-5)
 
 
 @pytest.mark.parametrize('B,H,Cc,Co', [(2, 24, 64, 3), (1, 17, 64, 3), (3, 40, 32, 1)])
-def test_final_projection_backward_with_four_pixels_in_flight_equals_the_default(cpulib, B, H, Cc, Co):
-    """conv1x1_to_nchw_bwd_kernel<4> (behind cd_conv_simt_set_preload): four pixels per trip, loads first; pixels are consumed in the
-    same order per thread -> dx, dW, db bit-identical"""
+def test_final_projection_backward_four_pixels_per_trip(cpulib, B, H, Cc, Co):
+    """conv1x1_to_nchw_bwd_kernel: four pixels per trip with their loads first, then one pixel per trip for the tail; the same
+    sums in the same order under both thread orders -> dx, dW, db bit-identical, and at fp32 accuracy against float64"""
     g = torch.Generator().manual_seed(B + H + Cc)
     x, dout = torch.randn(B, H, H, Cc, generator=g), torch.randn(B, Co, H, H, generator=g)
     w = torch.randn(Co, Cc, generator=g) / 8
     res = []
     for order in (0, 1):
         cpulib.simt_set_reverse_order(order)
-        for pre in (0, 1):
-            cpulib.cd_conv_simt_set_preload(pre)
-            dx, dw, db = torch.full((B, H, H, Cc), 7.0), torch.zeros(Co, Cc), torch.zeros(Co)
-            assert cpulib.cd_conv1x1_to_nchw_bwd(P(dout), P(x), Cc, B, H, H, Cc, P(w), Co, P(dx), Cc, P(dw), P(db), None) == 0
-            res.append(torch.cat([dx.reshape(-1), dw.reshape(-1), db.reshape(-1)]))
-    cpulib.cd_conv_simt_set_preload(0)
+        dx, dw, db = torch.full((B, H, H, Cc), 7.0), torch.zeros(Co, Cc), torch.zeros(Co)
+        assert cpulib.cd_conv1x1_to_nchw_bwd(P(dout), P(x), Cc, B, H, H, Cc, P(w), Co, P(dx), Cc, P(dw), P(db), None) == 0
+        res.append(torch.cat([dx.reshape(-1), dw.reshape(-1), db.reshape(-1)]))
     cpulib.simt_set_reverse_order(0)
-    assert torch.equal(res[0], res[1]) and torch.equal(res[2], res[3])
+    assert torch.equal(res[0], res[1])
     want_dx = torch.einsum('bohw,oc->bhwc', dout.double(), w.double())
     want_dw = torch.einsum('bohw,bhwc->oc', dout.double(), x.double())
     want = torch.cat([want_dx.reshape(-1), want_dw.reshape(-1), dout.double().sum(dim=(0, 2, 3))]).float()
     assert close(res[1], want, 1e-4)
 
 
-@pytest.mark.parametrize('B,rows,Cc,pad,out_ld', [(2, 1024, 64, 0, 80), (3, 300, 128, 8, 128), (1, 5000, 32, 0, 32), (2, 256, 512, 0, 600)])
+@pytest.mark.parametrize('B,rows,Cc,pad,out_ld', [(2, 1024, 64, 0, 80), (3, 300, 128, 8, 128), (1, 5000, 32, 0, 32), (2, 256, 512, 0, 600),
+                                                  (2, 200, 64, 0, 64), (2, 1024, 30, 2, 40), (2, 512, 64, 1, 64), (3, 2048, 128, 4, 136)])
 def test_batched_column_sums_float4_variant(cpulib, B, rows, Cc, pad, out_ld):
-    """colsum_batched_vec_kernel (behind cd_conv_simt_set_preload): float4 loads, four in flight; accumulates into `out` like the
-    scalar kernel, to fp32 rounding (another summation order)"""
+    """colsum_batched_vec_kernel (float4 loads, four in flight) where C % 4 == 0, ld % 4 == 0 and rows >= 256; the scalar
+    colsum_batched_kernel for fewer rows, other C or ld; both accumulate into `out`, to fp32 rounding of the float64 sums"""
     g = torch.Generator().manual_seed(rows + Cc)
     ld = Cc + pad
     x = torch.randn(B, rows, ld, generator=g)
     res = []
     for order in (0, 1):
         cpulib.simt_set_reverse_order(order)
-        for pre in (0, 1):
-            cpulib.cd_conv_simt_set_preload(pre)
-            out = torch.full((B, out_ld), 0.5)
-            assert cpulib.cd_colsum_batched(P(x), ld, B, ctypes_mod.c_int64(rows), Cc, P(out), out_ld, None) == 0
-            res.append(out)
-    cpulib.cd_conv_simt_set_preload(0)
+        out = torch.full((B, out_ld), 0.5)
+        assert cpulib.cd_colsum_batched(P(x), ld, B, ctypes_mod.c_int64(rows), Cc, P(out), out_ld, None) == 0
+        res.append(out)
     cpulib.simt_set_reverse_order(0)
     want = torch.full((B, out_ld), 0.5)
     want[:, :Cc] += x[:, :, :Cc].double().sum(dim=1).float()
