@@ -50,6 +50,17 @@ int cd_linattn_weff_staged(const float* ctx, const float* ksum, const float* w_o
 int cd_linattn_bwd_small_staged(const float* dweff, const float* ctx, const float* ksum, const float* w_out, int B, int dim,
                                 float scale, float* dw_out, float* dctxn, float* rowdot, cudaStream_t st);
 
+// elementwise.cu: split-plane GroupNorm, taken by cd_groupnorm_fwd / cd_groupnorm_bwd for planes of more than
+// CD_GN_SPLIT_MIN_HW pixels (smaller planes keep one CTA per image).  A chunk is GN_SPLIT_ITERS pixels per pixel lane of a
+// 512-thread CTA.  cd_gn_workspace returns a cached per-(device, stream) device buffer of at least `bytes`.  cd_gn_split_stats
+// leaves the per-chunk (mean, M2) partials in part[B][nch][groups][2] and (mean, rstd) of x + cond in stats[B][groups][2].
+constexpr long long CD_GN_SPLIT_MIN_HW = 128 * 128;
+constexpr int GN_SPLIT_ITERS = 16;
+int cd_gn_split_chunk(int C);
+int cd_gn_workspace(size_t bytes, cudaStream_t st, float** ws);
+int cd_gn_split_stats(const float* x, int x_ld, int B, long long HW, int C, int groups, const float* cond, int cond_ld, float eps,
+                      float* part, float* stats, cudaStream_t st);
+
 // linattn_bwd.cu: per-pixel LinearAttention backward on mma.sync; returns 1 when the CUDA-core kernel should run
 int cd_linattn_bwd_kv_mma(const float* qkv, int ld, int B, int n, const float* kmax, const float* ksum, const float* dctxn,
                           const float* rowdot, float* dqkv, int dld, cudaStream_t st);
@@ -86,6 +97,12 @@ __device__ __forceinline__ float cd_warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+// split-plane GroupNorm: pixels of chunk k (cp pixels) that pixel lane pl of np visits (pl, pl + np, ...; ragged last chunk)
+__device__ __forceinline__ int cd_gn_lane_count(long long HW, int k, int cp, int pl, int np) {
+  const long long rem = HW - static_cast<long long>(k) * cp;
+  if (rem >= cp) return GN_SPLIT_ITERS;
+  return pl < rem ? static_cast<int>((rem - pl + np - 1) / np) : 0;
 }
 __device__ __forceinline__ float cd_warp_max(float v) {
 #pragma unroll

@@ -3,6 +3,8 @@
 // MLP (DB:91-103,209-216,140-143), the LinearAttention softmax/context reduction (DB:176-187), the
 // final 1x1 projection to image channels (DB:253) and NCHW<->NHWC boundary conversion.
 #include "cd_common.cuh"
+#include <mutex>
+#include <vector>
 
 namespace {
 
@@ -955,12 +957,190 @@ time_mlp2_dense_kernel(const long long* __restrict__ t, int dim, int hid, int td
     if (lane == 0) temb[b * tdim + o] = a;
   }
 }
+
+// ---- GroupNorm split-plane path (planes above CD_GN_SPLIT_MIN_HW pixels): a (chunk x image) grid of CTAs with the thread ->
+// (pixel lane, channel quad) mapping of groupnorm_kernel; chunk k of image b covers pixels [k * cp, (k + 1) * cp), cp =
+// cd_gn_split_chunk(C) = GN_SPLIT_ITERS pixels per active thread.  Statistics are (count, mean, M2) triples merged with Chan's
+// formula in a fixed order (no E[x^2] - mean^2 cancellation for inputs with a large mean, no float atomics).
+// merge (nb, meanb, m2b) into (n, mean, m2)
+__device__ __forceinline__ void chan_merge(float& n, float& mean, float& m2, float nb, float meanb, float m2b) {
+  if (nb == 0.f) return;
+  const float nn = n + nb, d = meanb - mean;
+  mean += d * (nb / nn);
+  m2 += m2b + d * d * (n * nb / nn);
+  n = nn;
+}
+
+// fixed-order tree over the lanes of a warp; lane 0 ends with the merge of all 32
+__device__ __forceinline__ void chan_warp_merge(float& n, float& mean, float& m2) {
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float nb = __shfl_down_sync(0xffffffffu, n, o), mb = __shfl_down_sync(0xffffffffu, mean, o);
+    const float qb = __shfl_down_sync(0xffffffffu, m2, o);
+    if ((threadIdx.x & 31) + o < 32 && ((threadIdx.x & 31) & (2 * o - 1)) == 0) chan_merge(n, mean, m2, nb, mb, qb);
+  }
+}
+
+// pass 1: per-(image, chunk, group) (mean, M2) of x + cond -> part[b][k][g][2]; the count is implied by the chunk geometry.
+// Each thread keeps shifted sums about its first value (one chunk holds at most GN_SPLIT_ITERS values per thread-channel),
+// then one warp per group merges the thread-channel triples.
+__global__ void __launch_bounds__(512)
+gn_split_stats_kernel(const float* __restrict__ x, int x_ld, long long HW, int C, int groups, const float* __restrict__ cond,
+                      int cond_ld, int cp, float* __restrict__ part) {
+  __shared__ float tm[4][512], tq[4][512];
+  const int k = blockIdx.x, b = blockIdx.y, nch = gridDim.x;
+  const int nq = C >> 2, cg = C / groups;
+  const int q = threadIdx.x % nq, pl = threadIdx.x / nq, np = blockDim.x / nq;
+  const long long base = static_cast<long long>(b) * HW + static_cast<long long>(k) * cp;
+  if (pl < np) {
+    float4 cadd = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (cond) cadd = *reinterpret_cast<const float4*>(cond + static_cast<long long>(b) * cond_ld + q * 4);
+    const int cnt = cd_gn_lane_count(HW, k, cp, pl, np);
+    float sh[4] = {0.f, 0.f, 0.f, 0.f}, s[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll 4
+    for (int i = 0; i < cnt; ++i) {
+      float4 v = *reinterpret_cast<const float4*>(x + (base + pl + static_cast<long long>(i) * np) * x_ld + q * 4);
+      const float w[4] = {v.x + cadd.x, v.y + cadd.y, v.z + cadd.z, v.w + cadd.w};
+      if (i == 0) for (int j = 0; j < 4; ++j) sh[j] = w[j];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) { const float d = w[j] - sh[j]; s[j] += d; s2[j] += d * d; }
+    }
+    const float inv = cnt > 0 ? 1.f / static_cast<float>(cnt) : 0.f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      tm[j][threadIdx.x] = sh[j] + s[j] * inv;
+      tq[j][threadIdx.x] = fmaxf(s2[j] - s[j] * s[j] * inv, 0.f);
+    }
+  }
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  for (int g = warp; g < groups; g += nw) {
+    float n = 0.f, mean = 0.f, m2 = 0.f;
+    for (int e = lane; e < cg * np; e += 32) {           // entry e: channel g*cg + e/np of pixel lane e%np
+      const int c = g * cg + e / np, pp = e % np, t = pp * nq + (c >> 2);
+      chan_merge(n, mean, m2, static_cast<float>(cd_gn_lane_count(HW, k, cp, pp, np)), tm[c & 3][t], tq[c & 3][t]);
+    }
+    chan_warp_merge(n, mean, m2);
+    if (lane == 0) {
+      float* o = part + ((static_cast<long long>(b) * nch + k) * groups + g) * 2;
+      o[0] = mean; o[1] = m2;
+    }
+  }
+}
+
+// pass 2: merge the chunks of each (image, group) in a fixed order -> stats[b][g] = (mean, rstd); one warp per group
+__global__ void __launch_bounds__(256)
+gn_split_combine_kernel(const float* __restrict__ part, long long HW, int cg, int groups, int cp, int nch, float eps,
+                        float* __restrict__ stats) {
+  const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  for (int g = warp; g < groups; g += nw) {
+    float n = 0.f, mean = 0.f, m2 = 0.f;
+    for (int k = lane; k < nch; k += 32) {
+      const float* p = part + ((static_cast<long long>(b) * nch + k) * groups + g) * 2;
+      const long long pix = HW - static_cast<long long>(k) * cp < cp ? HW - static_cast<long long>(k) * cp : cp;
+      chan_merge(n, mean, m2, static_cast<float>(pix * cg), p[0], p[1]);
+    }
+    chan_warp_merge(n, mean, m2);
+    if (lane == 0) {
+      stats[(static_cast<long long>(b) * groups + g) * 2] = mean;
+      stats[(static_cast<long long>(b) * groups + g) * 2 + 1] = rsqrtf(m2 / n + eps);
+    }
+  }
+}
+
+// pass 3: y = (x + cond - mean) * rstd * gamma + beta [swish] over the (chunk x image) grid
+__global__ void __launch_bounds__(512)
+gn_split_norm_kernel(const float* __restrict__ x, int x_ld, long long HW, int C, int groups, const float* __restrict__ cond,
+                     int cond_ld, const float* __restrict__ gamma, const float* __restrict__ beta, int swish, int cp,
+                     const float* __restrict__ stats, float* __restrict__ y, int y_ld) {
+  const int k = blockIdx.x, b = blockIdx.y;
+  const int nq = C >> 2, cg = C / groups;
+  const int q = threadIdx.x % nq, pl = threadIdx.x / nq, np = blockDim.x / nq;
+  if (pl >= np) return;
+  float4 cadd = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (cond) cadd = *reinterpret_cast<const float4*>(cond + static_cast<long long>(b) * cond_ld + q * 4);
+  float mean[4], rstd[4];
+  for (int j = 0; j < 4; ++j) {
+    const float* st = stats + (static_cast<long long>(b) * groups + (q * 4 + j) / cg) * 2;
+    mean[j] = st[0]; rstd[j] = st[1];
+  }
+  const float4 gm = *reinterpret_cast<const float4*>(gamma + q * 4);
+  const float4 bt = *reinterpret_cast<const float4*>(beta + q * 4);
+  const long long base = static_cast<long long>(b) * HW + static_cast<long long>(k) * cp;
+  const int cnt = cd_gn_lane_count(HW, k, cp, pl, np);
+#pragma unroll 4
+  for (int i = 0; i < cnt; ++i) {
+    const long long p = base + pl + static_cast<long long>(i) * np;
+    float4 v = *reinterpret_cast<const float4*>(x + p * x_ld + q * 4);
+    float o[4] = {(v.x + cadd.x - mean[0]) * rstd[0] * gm.x + bt.x, (v.y + cadd.y - mean[1]) * rstd[1] * gm.y + bt.y,
+                  (v.z + cadd.z - mean[2]) * rstd[2] * gm.z + bt.z, (v.w + cadd.w - mean[3]) * rstd[3] * gm.w + bt.w};
+    if (swish) for (int j = 0; j < 4; ++j) o[j] = o[j] / (1.f + __expf(-o[j]));
+    *reinterpret_cast<float4*>(y + p * y_ld + q * 4) = make_float4(o[0], o[1], o[2], o[3]);
+  }
+}
 }  // namespace
+
+int cd_gn_split_chunk(int C) { return (512 / (C / 4)) * GN_SPLIT_ITERS; }
+
+int cd_gn_workspace(size_t bytes, cudaStream_t st, float** ws) {
+#ifdef CD_HOST_ONLY
+  static std::vector<float> buf;
+  if (buf.size() * sizeof(float) < bytes) buf.resize(bytes / sizeof(float) + 1);
+  *ws = buf.data();
+  return 0;
+#else
+  // one buffer per (device, stream), grown in stream order and never shrunk.  A buffer a CUDA graph has captured stays
+  // allocated for the life of the process (the graph may be replayed); growing one during a capture is refused.
+  struct Entry { int dev; cudaStream_t st; void* p; size_t bytes; bool captured; };
+  static std::mutex mu;
+  static std::vector<Entry> cache;
+  int dev = 0;
+  CD_CUDA(cudaGetDevice(&dev));
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CD_CUDA(cudaStreamIsCapturing(st, &cs));
+  std::lock_guard<std::mutex> lock(mu);
+  Entry* e = nullptr;
+  for (Entry& c : cache) if (c.dev == dev && c.st == st) e = &c;
+  if (!e) { cache.push_back(Entry{dev, st, nullptr, 0, false}); e = &cache.back(); }
+  if (e->bytes < bytes) {
+    CD_REQUIRE(cs == cudaStreamCaptureStatusNone, "cd_groupnorm: the split-plane path needs a %zu-byte workspace on this stream; "
+               "run the same shape once outside CUDA-graph capture first", bytes);
+    if (e->p && !e->captured) CD_CUDA(cudaFreeAsync(e->p, st));
+    e->p = nullptr; e->bytes = 0; e->captured = false;
+    CD_CUDA(cudaMallocAsync(&e->p, bytes, st));
+    e->bytes = bytes;
+  }
+  if (cs != cudaStreamCaptureStatusNone) e->captured = true;
+  *ws = static_cast<float*>(e->p);
+  return 0;
+#endif
+}
+
+int cd_gn_split_stats(const float* x, int x_ld, int B, long long HW, int C, int groups, const float* cond, int cond_ld, float eps,
+                      float* part, float* stats, cudaStream_t st) {
+  const int cp = cd_gn_split_chunk(C), nch = cd_cdiv(HW, cp);
+  gn_split_stats_kernel<<<dim3(nch, B), 512, 0, st>>>(x, x_ld, HW, C, groups, cond, cond_ld, cp, part);
+  CD_LAUNCH_CHECK();
+  gn_split_combine_kernel<<<B, 256, 0, st>>>(part, HW, C / groups, groups, cp, nch, eps, stats);
+  CD_LAUNCH_CHECK();
+  return 0;
+}
 
 extern "C" int cd_groupnorm_fwd(const float* x, int x_ld, int B, int64_t HW, int C, int groups, const float* cond, int cond_ld,
                                 const float* gamma, const float* beta, float eps, int swish, float* y, int y_ld, void* stream) {
   CD_REQUIRE(C % 4 == 0 && C % groups == 0 && C / 4 <= 512 && x_ld % 4 == 0 && y_ld % 4 == 0 && (!cond || cond_ld % 4 == 0),
              "cd_groupnorm_fwd: unsupported C=%d groups=%d", C, groups);
+  if (HW > CD_GN_SPLIT_MIN_HW) {
+    CD_REQUIRE(B <= 65535, "cd_groupnorm_fwd: the split-plane path takes at most 65535 images (B=%d)", B);
+    const long long nch = cd_cdiv(HW, cd_gn_split_chunk(C)), nstat = 2LL * B * groups;
+    float* ws = nullptr;
+    if (int rc = cd_gn_workspace(sizeof(float) * (nstat + nstat * nch), static_cast<cudaStream_t>(stream), &ws)) return rc;
+    if (int rc = cd_gn_split_stats(x, x_ld, B, HW, C, groups, cond, cond_ld, eps, ws + nstat, ws, static_cast<cudaStream_t>(stream))) return rc;
+    gn_split_norm_kernel<<<dim3(nch, B), 512, 0, static_cast<cudaStream_t>(stream)>>>(x, x_ld, HW, C, groups, cond, cond_ld, gamma, beta,
+                                                                                        swish, cd_gn_split_chunk(C), ws, y, y_ld);
+    CD_LAUNCH_CHECK();
+    return 0;
+  }
   groupnorm_kernel<<<B, 512, sizeof(float) * (2 * groups + 8 * 512), static_cast<cudaStream_t>(stream)>>>(x, x_ld, (int)HW, C, groups, cond, cond_ld,
                                                                                            gamma, beta, eps, swish, y, y_ld);
   CD_LAUNCH_CHECK();

@@ -106,6 +106,156 @@ groupnorm_bwd_kernel(const float* __restrict__ x, int x_ld, int HW, int C, int g
   }
 }
 
+// ---- split-plane backward (planes above CD_GN_SPLIT_MIN_HW pixels; the (chunk x image) grid and thread mapping of the
+// forward's gn_split_* kernels in elementwise.cu).  Every per-channel sum is formed per chunk and the chunks are added in a
+// fixed order: no float atomics, run-to-run identical results.
+// per-channel sum over the pixel lanes of a CTA in lane order: v[j][pp * nq + c / 4] holds channel c of pixel lane pp
+__device__ __forceinline__ float gn_lane_sum(const float (*v)[512], int c, int nq, int np) {
+  float a = 0.f;
+  for (int pp = 0; pp < np; ++pp) a += v[c & 3][pp * nq + (c >> 2)];
+  return a;
+}
+
+// out[c] = sum over k < nch of src[k * stride + c] in a fixed order: slice s of nsl = max(1, blockDim / C) adds k = s, s + nsl,
+// ..., then the slices are added in order.  scratch holds nsl * C <= 2048 floats.
+__device__ void gn_chunk_colsum(const float* __restrict__ src, long long stride, int nch, int C, float* scratch, float* out) {
+  const int nsl = C < static_cast<int>(blockDim.x) ? blockDim.x / C : 1;
+  for (int i = threadIdx.x; i < nsl * C; i += blockDim.x) {
+    const int c = i % C, s = i / C;
+    float a = 0.f;
+    for (int k = s; k < nch; k += nsl) a += src[k * stride + c];
+    scratch[i] = a;
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float a = 0.f;
+    for (int s = 0; s < nsl; ++s) a += scratch[s * C + c];
+    out[c] = a;
+  }
+  __syncthreads();
+}
+
+// per-(image, chunk, channel) sums of dz and dz*xh -> bpart[b][k][2][C]
+__global__ void __launch_bounds__(512)
+gn_split_bwd_sums_kernel(const float* __restrict__ x, int x_ld, long long HW, int C, int groups, const float* __restrict__ cond,
+                         int cond_ld, const float* __restrict__ gamma, const float* __restrict__ beta, int swish,
+                         const float* __restrict__ dy, int dy_ld, int cp, const float* __restrict__ stats, float* __restrict__ bpart) {
+  __shared__ float tz[4][512], tzx[4][512];
+  const int k = blockIdx.x, b = blockIdx.y, nch = gridDim.x;
+  const int nq = C >> 2, cg = C / groups;
+  const int q = threadIdx.x % nq, pl = threadIdx.x / nq, np = blockDim.x / nq;
+  if (pl < np) {
+    float cadd[4] = {0.f, 0.f, 0.f, 0.f}, mean[4], rstd[4], gm[4], bt[4];
+    if (cond) { const float4 cv = *reinterpret_cast<const float4*>(cond + static_cast<long long>(b) * cond_ld + q * 4); cadd[0] = cv.x; cadd[1] = cv.y; cadd[2] = cv.z; cadd[3] = cv.w; }
+    for (int j = 0; j < 4; ++j) {
+      const float* st = stats + (static_cast<long long>(b) * groups + (q * 4 + j) / cg) * 2;
+      mean[j] = st[0]; rstd[j] = st[1]; gm[j] = gamma[q * 4 + j]; bt[j] = beta[q * 4 + j];
+    }
+    float sdz[4] = {0.f, 0.f, 0.f, 0.f}, sdzx[4] = {0.f, 0.f, 0.f, 0.f};
+    const long long base = static_cast<long long>(b) * HW + static_cast<long long>(k) * cp + pl;
+    const int cnt = cd_gn_lane_count(HW, k, cp, pl, np);
+    for (int i = 0; i < cnt; ++i) {
+      const long long p = base + static_cast<long long>(i) * np;
+      const float4 v4 = *reinterpret_cast<const float4*>(x + p * x_ld + q * 4);
+      const float4 d4 = *reinterpret_cast<const float4*>(dy + p * dy_ld + q * 4);
+      const float v[4] = {v4.x + cadd[0], v4.y + cadd[1], v4.z + cadd[2], v4.w + cadd[3]};
+      const float d[4] = {d4.x, d4.y, d4.z, d4.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float xh = (v[j] - mean[j]) * rstd[j];
+        const float dz = swish ? d[j] * swish_grad(xh * gm[j] + bt[j]) : d[j];
+        sdz[j] += dz; sdzx[j] += dz * xh;
+      }
+    }
+    for (int j = 0; j < 4; ++j) { tz[j][threadIdx.x] = sdz[j]; tzx[j][threadIdx.x] = sdzx[j]; }
+  }
+  __syncthreads();
+  float* o = bpart + (static_cast<long long>(b) * nch + k) * 2 * C;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) { o[c] = gn_lane_sum(tz, c, nq, np); o[C + c] = gn_lane_sum(tzx, c, nq, np); }
+}
+
+// per image: chunk sums -> csum[b][2][C] (dz, dz*xh) and the group means of gamma*dz and gamma*dz*xh -> gab[b][groups][2]
+__global__ void __launch_bounds__(512)
+gn_split_bwd_reduce_kernel(const float* __restrict__ bpart, int nch, int C, int groups, const float* __restrict__ gamma, float inv_n,
+                           float* __restrict__ csum, float* __restrict__ gab) {
+  __shared__ float scratch[2048], cz[2048], czx[2048];
+  const int b = blockIdx.x, cg = C / groups;
+  const float* src = bpart + static_cast<long long>(b) * nch * 2 * C;
+  gn_chunk_colsum(src, 2LL * C, nch, C, scratch, cz);
+  gn_chunk_colsum(src + C, 2LL * C, nch, C, scratch, czx);
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    csum[static_cast<long long>(b) * 2 * C + c] = cz[c];
+    csum[static_cast<long long>(b) * 2 * C + C + c] = czx[c];
+  }
+  for (int g = threadIdx.x; g < groups; g += blockDim.x) {
+    float a = 0.f, a2 = 0.f;
+    for (int c = g * cg; c < (g + 1) * cg; ++c) { a += gamma[c] * cz[c]; a2 += gamma[c] * czx[c]; }
+    gab[(static_cast<long long>(b) * groups + g) * 2] = a * inv_n;
+    gab[(static_cast<long long>(b) * groups + g) * 2 + 1] = a2 * inv_n;
+  }
+}
+
+// dx over the (chunk x image) grid; with dpart, also the per-(image, chunk, channel) sums of dx -> dpart[b][k][C]
+__global__ void __launch_bounds__(512)
+gn_split_bwd_dx_kernel(const float* __restrict__ x, int x_ld, long long HW, int C, int groups, const float* __restrict__ cond,
+                       int cond_ld, const float* __restrict__ gamma, const float* __restrict__ beta, int swish,
+                       const float* __restrict__ dy, int dy_ld, int cp, const float* __restrict__ stats,
+                       const float* __restrict__ gab, float* __restrict__ dx, int dx_ld, float* __restrict__ dpart) {
+  __shared__ float tdx[4][512];
+  const int k = blockIdx.x, b = blockIdx.y, nch = gridDim.x;
+  const int nq = C >> 2, cg = C / groups;
+  const int q = threadIdx.x % nq, pl = threadIdx.x / nq, np = blockDim.x / nq;
+  if (pl < np) {
+    float cadd[4] = {0.f, 0.f, 0.f, 0.f}, mean[4], rstd[4], gm[4], bt[4], ma[4], mb[4], sdx[4] = {0.f, 0.f, 0.f, 0.f};
+    if (cond) { const float4 cv = *reinterpret_cast<const float4*>(cond + static_cast<long long>(b) * cond_ld + q * 4); cadd[0] = cv.x; cadd[1] = cv.y; cadd[2] = cv.z; cadd[3] = cv.w; }
+    for (int j = 0; j < 4; ++j) {
+      const long long g = static_cast<long long>(b) * groups + (q * 4 + j) / cg;
+      mean[j] = stats[g * 2]; rstd[j] = stats[g * 2 + 1]; ma[j] = gab[g * 2]; mb[j] = gab[g * 2 + 1];
+      gm[j] = gamma[q * 4 + j]; bt[j] = beta[q * 4 + j];
+    }
+    const long long base = static_cast<long long>(b) * HW + static_cast<long long>(k) * cp + pl;
+    const int cnt = cd_gn_lane_count(HW, k, cp, pl, np);
+#pragma unroll 4
+    for (int i = 0; i < cnt; ++i) {
+      const long long p = base + static_cast<long long>(i) * np;
+      const float4 v4 = *reinterpret_cast<const float4*>(x + p * x_ld + q * 4);
+      const float4 d4 = *reinterpret_cast<const float4*>(dy + p * dy_ld + q * 4);
+      const float v[4] = {v4.x + cadd[0], v4.y + cadd[1], v4.z + cadd[2], v4.w + cadd[3]};
+      const float d[4] = {d4.x, d4.y, d4.z, d4.w};
+      float o[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float xh = (v[j] - mean[j]) * rstd[j];
+        const float dz = swish ? d[j] * swish_grad(xh * gm[j] + bt[j]) : d[j];
+        o[j] = rstd[j] * (dz * gm[j] - ma[j] - xh * mb[j]);
+        sdx[j] += o[j];
+      }
+      *reinterpret_cast<float4*>(dx + p * dx_ld + q * 4) = make_float4(o[0], o[1], o[2], o[3]);
+    }
+    for (int j = 0; j < 4; ++j) tdx[j][threadIdx.x] = sdx[j];
+  }
+  if (!dpart) return;
+  __syncthreads();
+  for (int c = threadIdx.x; c < C; c += blockDim.x) dpart[(static_cast<long long>(b) * nch + k) * C + c] = gn_lane_sum(tdx, c, nq, np);
+}
+
+// blocks b < B (with dcond): dcond[b][c] = sum over chunks of dpart; the last block: dgamma / dbeta += sum over images of csum
+__global__ void __launch_bounds__(512)
+gn_split_bwd_final_kernel(const float* __restrict__ csum, int B, int C, const float* __restrict__ dpart, int nch,
+                          float* __restrict__ dcond, int dcond_ld, float* __restrict__ dgamma, float* __restrict__ dbeta) {
+  __shared__ float scratch[2048];
+  const int b = blockIdx.x;
+  if (b == static_cast<int>(gridDim.x) - 1) {
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+      float a = 0.f, a2 = 0.f;
+      for (int i = 0; i < B; ++i) { a += csum[static_cast<long long>(i) * 2 * C + c]; a2 += csum[static_cast<long long>(i) * 2 * C + C + c]; }
+      dbeta[c] += a; dgamma[c] += a2;
+    }
+    return;
+  }
+  gn_chunk_colsum(dpart + static_cast<long long>(b) * nch * C, C, nch, C, scratch, dcond + static_cast<long long>(b) * dcond_ld);
+}
+
 // counter-based mask: keep element i of the call `seed` with probability 1-p (murmur3 finaliser of (seed, i))
 __device__ __forceinline__ float uniform01(unsigned long long seed, unsigned long long i) {
   unsigned long long h = seed ^ (i * 0x9E3779B97F4A7C15ull);
@@ -230,6 +380,29 @@ extern "C" int cd_groupnorm_bwd(const float* x, int x_ld, int B, int64_t HW, int
                                 float* dx, int dx_ld, float* dgamma, float* dbeta, float* dcond, int dcond_ld, void* stream) {
   CD_REQUIRE(C % 4 == 0 && C % groups == 0 && C / 4 <= 512 && x_ld % 4 == 0 && dy_ld % 4 == 0 && dx_ld % 4 == 0 &&
              (!cond || cond_ld % 4 == 0), "cd_groupnorm_bwd: unsupported C=%d groups=%d", C, groups);
+  if (HW > CD_GN_SPLIT_MIN_HW) {
+    CD_REQUIRE(B <= 65535, "cd_groupnorm_bwd: the split-plane path takes at most 65535 images (B=%d)", B);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int cp = cd_gn_split_chunk(C), nch = cd_cdiv(HW, cp);
+    // workspace: stats | part | gab | csum | bpart | dpart
+    const long long nstat = 2LL * B * groups, nc = static_cast<long long>(B) * C;
+    float* ws = nullptr;
+    if (int rc = cd_gn_workspace(sizeof(float) * (nstat * (2 + nch) + nc * (2 + 2LL * nch + (dcond ? nch : 0))), st, &ws)) return rc;
+    float *stats = ws, *part = stats + nstat, *gab = part + nstat * nch, *csum = gab + nstat, *bpart = csum + 2 * nc;
+    float* dpart = dcond ? bpart + 2 * nc * nch : nullptr;
+    if (int rc = cd_gn_split_stats(x, x_ld, B, HW, C, groups, cond, cond_ld, eps, part, stats, st)) return rc;
+    gn_split_bwd_sums_kernel<<<dim3(nch, B), 512, 0, st>>>(x, x_ld, HW, C, groups, cond, cond_ld, gamma, beta, swish, dy, dy_ld, cp,
+                                                           stats, bpart);
+    CD_LAUNCH_CHECK();
+    gn_split_bwd_reduce_kernel<<<B, 512, 0, st>>>(bpart, nch, C, groups, gamma, 1.f / (static_cast<float>(HW) * (C / groups)), csum, gab);
+    CD_LAUNCH_CHECK();
+    gn_split_bwd_dx_kernel<<<dim3(nch, B), 512, 0, st>>>(x, x_ld, HW, C, groups, cond, cond_ld, gamma, beta, swish, dy, dy_ld, cp,
+                                                         stats, gab, dx, dx_ld, dpart);
+    CD_LAUNCH_CHECK();
+    gn_split_bwd_final_kernel<<<dcond ? B + 1 : 1, 512, 0, st>>>(csum, B, C, dpart, nch, dcond, dcond_ld, dgamma, dbeta);
+    CD_LAUNCH_CHECK();
+    return 0;
+  }
   const size_t smem = sizeof(float) * (4 * groups + 3 * C);
   groupnorm_bwd_kernel<<<B, 512, smem, static_cast<cudaStream_t>(stream)>>>(x, x_ld, (int)HW, C, groups, cond, cond_ld, gamma, beta, eps, swish,
                                                                          dy, dy_ld, dx, dx_ld, dgamma, dbeta, dcond, dcond_ld);

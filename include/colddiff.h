@@ -12,7 +12,8 @@
  *
  * Conventions
  *   - plain pointers and sizes only; all pointers are DEVICE pointers unless named host_*;
- *   - the library never allocates device memory and never synchronises: the caller passes
+ *   - the library never synchronises, and allocates device memory only for the split-plane GroupNorm
+ *     partials (a per-(device, stream) cached buffer, see cd_groupnorm_fwd): otherwise the caller passes
  *     outputs/workspaces (torch caching allocator) and a cudaStream_t (as void*);
  *   - return value: 0 = ok, <0 = error (text via cd_last_error); no exceptions cross the ABI;
  *   - activations inside the engine are NHWC fp32 ("pixel rows" of `ld` floats, channel slice
@@ -338,7 +339,10 @@ int cd_snow_layers(const double* noise, int SB, int ch, int m, int trim, int H, 
  * convolutions (3x3, 1x1 q/k/v/proj/nin_shortcut, asymmetric-pad stride-2 Downsample, and the two batched matmuls of AttnBlock
  * as per-batch-weight 1x1 tap-list convolutions) run through cd_conv_fwd.
  * ------------------------------------------------------------------------------------------ */
-/* GroupNorm(groups, eps) of (x + cond[b,c]) [* swish] on NHWC (M2:32-33, 114-123) */
+/* GroupNorm(groups, eps) of (x + cond[b,c]) [* swish] on NHWC (M2:32-33, 114-123).  HW <= 128*128: one CTA per image.
+ * Larger planes: a (pixel chunk x image) grid with Chan-merged statistics and fixed-order sums (cd_groupnorm_bwd too); its
+ * partials go to a device buffer cached per (device, stream) that grows outside CUDA-graph capture only (a capture that
+ * would need it larger fails: run the shape once before capturing).  Needs C % 4 == 0, C / 4 <= 512 and B <= 65535. */
 int cd_groupnorm_fwd(const float* x, int x_ld, int B, int64_t HW, int C, int groups, const float* cond, int cond_ld,
                      const float* gamma, const float* beta, float eps, int swish, float* y, int y_ld, void* stream);
 /* in-place softmax(scale * s) over the last dimension of [rows][n] (M2:172-175) */
