@@ -57,7 +57,7 @@ if os.environ.get('COLDDIFF_2CTA') in ('0', '1', '2'):   # SM-pair (two-CTA clus
 lib.cd_last_error.argtypes = [C.c_char_p, C.c_size_t]
 if os.environ.get('COLDDIFF_CONV_TWO_CTAS') in ('0', '64', '128', '192'):   # two CTAs per SM for the N <= 128 convolution tiles (bit mask)
     lib.cd_conv_tc_set_two_ctas(int(os.environ['COLDDIFF_CONV_TWO_CTAS']))
-if os.environ.get('COLDDIFF_CONV_HALO') in ('0', '1', '2', '6', '8'):   # 3x3 convolution kernel: 0 shape-based (default), 1 / 2 / 6 shared-row kernel, 8 per-tap kernel
+if os.environ.get('COLDDIFF_CONV_HALO') in ('0', '1', '2', '4', '6', '8'):   # 3x3 convolution kernel: 0 shape-based (default), 1 / 2 / 6 shared-row kernel (16 x 8), 4 (16 x 16), 8 per-tap kernel
     lib.cd_conv_tc_set_halo(int(os.environ['COLDDIFF_CONV_HALO']))
 if os.environ.get('COLDDIFF_WGRAD_MODE') in ('0', '1', '8'):   # tensor-core weight gradient: 1 wgmma kernel where eligible (default), 8 mma.sync halo kernel, 0 mma.sync one X tile per tap
     lib.cd_wgrad_tc_set_mode(int(os.environ['COLDDIFF_WGRAD_MODE']))

@@ -262,6 +262,46 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
 constexpr int kRowsTW = 16, kRowsTH = kTileM / kRowsTW;
 constexpr int kRowsBoxBytes = kRowsTW * (kRowsTH + 2) * 128;     // 20 KB: one tap column of one chunk
 
+// TMA producer of both shared-row kernels (one elected thread of the producer warp): per tile of kRowsTW x TH pixels, source and
+// 32-channel chunk, one box {32 ch, kRowsTW, TH + 2, 1} per tap column into the ABOXES-deep box ring, each followed by the weight
+// tiles of that column's taps into the STAGES-deep weight ring
+template <int BN, int TH, int ABOXES, int STAGES>
+__device__ __forceinline__ void rows_producer(const CUtensorMap& mapA0, const CUtensorMap& mapA1, const CUtensorMap& mapB0,
+                                              const CUtensorMap& mapB1, const TcParams& p, uint8_t* abox, uint8_t* wtile,
+                                              uint64_t* afull, uint64_t* aempty, uint64_t* full_bar, uint64_t* empty_bar) {
+  constexpr int kBBytes = BN * 128;
+  constexpr int kBoxBytes = kRowsTW * (TH + 2) * 128;
+  if (elect_one()) {
+    uint32_t stage = 0, ph = 0, ai = 0, aph = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      const int co0 = (tile % p.tiles_co) * BN;
+      int mt = tile / p.tiles_co;
+      const int x0 = (mt % p.tiles_x) * kRowsTW; mt /= p.tiles_x;
+      const int y0 = (mt % p.tiles_y) * TH;
+      const int n = mt / p.tiles_y;
+      for (int s = 0; s < p.nsrc; ++s) {
+        const CUtensorMap* mA = s ? &mapA1 : &mapA0;
+        const CUtensorMap* mB = s ? &mapB1 : &mapB0;
+        for (int kc = 0; kc < p.kchunks[s]; ++kc) {
+          for (int b = 0, i = 0; b < p.nbox[s]; ++b) {
+            mbar_wait(&aempty[ai], aph ^ 1u);
+            mbar_expect_tx(&afull[ai], kBoxBytes);
+            tma_load_4d(smem_u32(abox + ai * kBoxBytes), mA, &afull[ai], kc * kChunkK, x0 + p.boxdx[s][b], y0 - 1, n);
+            if (++ai == ABOXES) { ai = 0; aph ^= 1u; }
+            for (; i < p.boxend[s][b]; ++i) {
+              mbar_wait(&empty_bar[stage], ph ^ 1u);
+              mbar_expect_tx(&full_bar[stage], kBBytes);
+              tma_load_3d(smem_u32(wtile + stage * kBBytes), mB, &full_bar[stage], kc * kChunkK, co0, p.taporder[s][i]);
+              if (++stage == STAGES) { stage = 0; ph ^= 1u; }
+            }
+          }
+        }
+      }
+    }
+  }
+  __syncwarp();
+}
+
 template <int BN, int ABOXES, int STAGES, int CTAS>
 __global__ void __launch_bounds__(kThreads, CTAS)
 conv_rows_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
@@ -287,36 +327,7 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constan
   __syncthreads();
 
   if (warp == kConsumerWarps) {
-    // ===================== TMA producer: ONE elected thread =====================
-    if (elect_one()) {
-      uint32_t stage = 0, ph = 0, ai = 0, aph = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int co0 = (tile % p.tiles_co) * BN;
-        int mt = tile / p.tiles_co;
-        const int x0 = (mt % p.tiles_x) * kRowsTW; mt /= p.tiles_x;
-        const int y0 = (mt % p.tiles_y) * kRowsTH;
-        const int n = mt / p.tiles_y;
-        for (int s = 0; s < p.nsrc; ++s) {
-          const CUtensorMap* mA = s ? &mapA1 : &mapA0;
-          const CUtensorMap* mB = s ? &mapB1 : &mapB0;
-          for (int kc = 0; kc < p.kchunks[s]; ++kc) {
-            for (int b = 0, i = 0; b < p.nbox[s]; ++b) {
-              mbar_wait(&aempty[ai], aph ^ 1u);
-              mbar_expect_tx(&afull[ai], kRowsBoxBytes);
-              tma_load_4d(smem_u32(abox + ai * kRowsBoxBytes), mA, &afull[ai], kc * kChunkK, x0 + p.boxdx[s][b], y0 - 1, n);
-              if (++ai == ABOXES) { ai = 0; aph ^= 1u; }
-              for (; i < p.boxend[s][b]; ++i) {
-                mbar_wait(&empty_bar[stage], ph ^ 1u);
-                mbar_expect_tx(&full_bar[stage], kBBytes);
-                tma_load_3d(smem_u32(wtile + stage * kBBytes), mB, &full_bar[stage], kc * kChunkK, co0, p.taporder[s][i]);
-                if (++stage == STAGES) { stage = 0; ph ^= 1u; }
-              }
-            }
-          }
-        }
-      }
-    }
-    __syncwarp();
+    rows_producer<BN, kRowsTH, ABOXES, STAGES>(mapA0, mapA1, mapB0, mapB1, p, abox, wtile, afull, aempty, full_bar, empty_bar);
     return;
   }
 
@@ -376,6 +387,213 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constan
 }
 
 // ---------------------------------------------------------------------------------------------
+// Shared-row kernel with 16 x 16 pixel tiles: the problems, boxes and mainloop order of conv_rows_kernel, but a CTA tile is 256
+// output pixels of one image by BN output channels at one CTA per SM, so every weight tile serves twice as many pixels.  Warpgroup
+// w owns pixel rows 8 w .. 8 w + 7 (GEMM rows [128 w, 128 w + 128)) and issues two m64nBNk8 wgmmas per k step, one per 64-row
+// half h.  Both warpgroups read the same weight tile and the same box {32 ch, 16, 16 + 2, 1}; tap (dy, dx) of half h of warpgroup
+// w starts at byte (dy + 1) * 2 KB + w * 16 KB + h * 8 KB of its column's box, a whole number of SW128 atoms.  Every output
+// element goes through the same wgmma sequence as in conv_rows_kernel, so the two kernels agree bit for bit.
+// Epilogue: per 32-channel slice each warpgroup writes out (and out2) of its 128 pixels into SWIZZLE_128B staging slices, and one
+// of its threads stores them with TMA tensor stores (the maps' bounds clip ragged tiles and Cout).  The consumers go on into the
+// next tile's mainloop while the stores drain -- the overlap that the 16 x 8 kernel gets from two CTAs per SM.
+// ---------------------------------------------------------------------------------------------
+constexpr int kR256TH = 16;
+constexpr int kR256BoxBytes = kRowsTW * (kR256TH + 2) * 128;     // 36 KB: one tap column of one chunk
+constexpr int kR256Slice = 128 * 128;                            // staging: 128 pixels x 32 fp32 channels = 16 KB
+// warpgroup 0 = producer (warp 0 issues the TMA loads), warpgroups 1-2 = consumers.  Two 64 x BN accumulators per consumer thread
+// do not fit the 168 registers of 384 threads, so setmaxnreg moves registers from the producer to the consumers.
+constexpr int kR256Threads = 384;
+constexpr int kR256RegsLow = 40, kR256RegsHigh = 232;          // 128 x 40 + 256 x 232 <= 64 K registers
+
+// channels (col, col + 1) of one row of an epilogue operand, as far as they lie below Cout and `ok` (zeros elsewhere: those outputs
+// are clipped by the store)
+__device__ __forceinline__ float2 ld_pair(const float* row, int col, int Cout, bool ok) {
+  if (ok && col + 1 < Cout) return *reinterpret_cast<const float2*>(row + col);
+  if (ok && col < Cout) return make_float2(row[col], 0.f);
+  return make_float2(0.f, 0.f);
+}
+
+template <int BN, int ABOXES, int STAGES>
+__global__ void __launch_bounds__(kR256Threads, 1)
+conv_rows256_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
+                    const __grid_constant__ CUtensorMap mapB0, const __grid_constant__ CUtensorMap mapB1,
+                    const __grid_constant__ CUtensorMap mapO, const __grid_constant__ CUtensorMap mapO2, const __grid_constant__ TcParams p) {
+  constexpr int kBBytes = BN * 128;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
+  uint8_t* abox = smem;                                    // ABOXES activation boxes
+  uint8_t* wtile = smem + ABOXES * kR256BoxBytes;          // STAGES weight tiles
+  uint8_t* stg = wtile + STAGES * kBBytes;                 // per warpgroup: out slice, out2 slice
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stg + 4 * kR256Slice);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + STAGES;
+  uint64_t* afull = bars + 2 * STAGES;
+  uint64_t* aempty = bars + 2 * STAGES + ABOXES;
+  static_assert(2 * (STAGES + ABOXES) * 8 <= 256, "barrier block is 256 bytes");
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumerWarps); }
+    for (int i = 0; i < ABOXES; ++i) { mbar_init(&afull[i], 1); mbar_init(&aempty[i], kConsumerWarps); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(kR256RegsLow));
+    if (warp == 0)
+      rows_producer<BN, kR256TH, ABOXES, STAGES>(mapA0, mapA1, mapB0, mapB1, p, abox, wtile, afull, aempty, full_bar, empty_bar);
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(kR256RegsHigh));
+
+  // ===================== consumers: warpgroup 1 + cw owns GEMM rows [128 cw, 128 cw + 128); row m = pixel (m % 16, m / 16) =====================
+  const int cw = wg - 1;
+  const int tid = threadIdx.x & 127;
+  const int rl = (tid >> 5) * 16 + (lane >> 2);
+  const int q2 = (lane & 3) * 2;
+  const bool storer = tid == 0;                            // issues (and waits for) the warpgroup's bulk stores
+  uint8_t* so = stg + cw * 2 * kR256Slice;
+  uint8_t* so2 = so + kR256Slice;
+  auto release = [&](uint64_t* bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
+  auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" :: "r"(1 + cw) : "memory"); };
+  float acc[2][BN / 2];
+  uint32_t stage = 0, ph = 0, ai = 0, aph = 0;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    int k = 0;
+    uint32_t prev = 0, prev_a = 0;
+    for (int s = 0; s < p.nsrc; ++s) {
+      for (int kc = 0; kc < p.kchunks[s]; ++kc) {
+        for (int b = 0, i = 0; b < p.nbox[s]; ++b) {
+          mbar_wait(&afull[ai], aph);
+          const uint32_t abase = smem_u32(abox + ai * kR256BoxBytes) + cw * kABytes;
+          for (const int i0 = i; i < p.boxend[s][b]; ++i, ++k) {
+            mbar_wait(&full_bar[stage], ph);
+            wgmma_fence();
+            const uint64_t da0 = make_kmajor_sw128_desc(abase + p.tapoff[s][i]);
+            const uint64_t da1 = make_kmajor_sw128_desc(abase + p.tapoff[s][i] + kABytes / 2);
+            const uint64_t db = make_kmajor_sw128_desc(smem_u32(wtile + stage * kBBytes));
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+              wgmma_tf32<BN>(acc[0], da0 + uint64_t(kk * 2), db + uint64_t(kk * 2), (k | kk) != 0 ? 1u : 0u);
+              wgmma_tf32<BN>(acc[1], da1 + uint64_t(kk * 2), db + uint64_t(kk * 2), (k | kk) != 0 ? 1u : 0u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                         // the previous tap's MMAs have retired
+            if (k > 0) release(&empty_bar[prev]);
+            if (k > 0 && i == i0) release(&aempty[prev_a]);   // ... and with them every tap of the previous box
+            prev = stage;
+            if (++stage == STAGES) { stage = 0; ph ^= 1u; }
+          }
+          prev_a = ai;
+          if (++ai == ABOXES) { ai = 0; aph ^= 1u; }
+        }
+      }
+    }
+    wgmma_wait<0>();
+    if (k > 0) { release(&empty_bar[prev]); release(&aempty[prev_a]); }
+
+    const int co0 = (tile % p.tiles_co) * BN;
+    int mt = tile / p.tiles_co;
+    const int x0 = (mt % p.tiles_x) * kRowsTW; mt /= p.tiles_x;
+    const int yw = (mt % p.tiles_y) * kR256TH + 8 * cw;    // first pixel row of this warpgroup
+    const int n = mt / p.tiles_y;
+    if (yw >= p.Hg) continue;                              // ragged grid: no pixel of this warpgroup lies inside
+    // local row r = 64 h + rl + 8 e (e: acc[4 j + 2 e], acc[4 j + 2 e + 1]) is pixel (x0 + r % 16, yw + r / 16)
+    long long pix[2][2];
+    bool valid[2][2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int r = 64 * h + rl + 8 * e, gx = x0 + r % kRowsTW, gy = yw + r / kRowsTW;
+        valid[h][e] = gx < p.Wg && gy < p.Hg;
+        pix[h][e] = (static_cast<long long>(n) * p.Hg + gy) * p.Wg + gx;
+      }
+#pragma unroll
+    for (int c = 0; c < BN / 32; ++c) {
+      if (co0 + 32 * c >= p.Cout) break;
+      if (storer) bulk_wait_read<0>();                     // the previous stores have read the staging slices
+      wg_sync();
+      // epi_pair's arithmetic, one step at a time over the 8 column pairs of each half h of the slice: the branches on the epilogue
+      // operands stay outside the element loops, so the 8 independent chains (and their resid / aux loads) overlap
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float2 v[2][4];
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) v[e][jj] = make_float2(acc[h][16 * c + 4 * jj + 2 * e], acc[h][16 * c + 4 * jj + 2 * e + 1]);
+        if (p.bias) {
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const float2 b = ld_pair(p.bias, co0 + 32 * c + 8 * jj + q2, p.Cout, true);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) { v[e][jj].x += b.x; v[e][jj].y += b.y; }
+          }
+        }
+        if (p.resid) {
+          float2 r[2][4];
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) r[e][jj] = ld_pair(p.resid + pix[h][e] * p.resid_ld, co0 + 32 * c + 8 * jj + q2, p.Cout, valid[h][e]);
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) { v[e][jj].x += r[e][jj].x; v[e][jj].y += r[e][jj].y; }
+        }
+        // SWIZZLE_128B staging: the 16-byte chunk (8 jj + q2) / 4 of local row rr lands at chunk ^ (rr % 8)
+        auto soff = [&](int e, int jj) {
+          const int rr = 64 * h + rl + 8 * e;
+          return rr * 128 + ((((8 * jj + q2) >> 2) ^ (rr & 7)) << 4) + (q2 & 3) * 4;
+        };
+        if (p.out2) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) *reinterpret_cast<float2*>(so2 + soff(e, jj)) = v[e][jj];
+        }
+        if (p.act == CD_ACT_GELU) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) { v[e][jj].x = cd_gelu(v[e][jj].x); v[e][jj].y = cd_gelu(v[e][jj].y); }
+        } else if (p.act == CD_ACT_GELU_BWD) {
+          float2 a[2][4];
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) a[e][jj] = ld_pair(p.aux + pix[h][e] * p.aux_ld, co0 + 32 * c + 8 * jj + q2, p.Cout, valid[h][e]);
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) { v[e][jj].x *= cd_gelu_grad(a[e][jj].x); v[e][jj].y *= cd_gelu_grad(a[e][jj].y); }
+        }
+        if (p.round_tf32) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) { v[e][jj].x = cd_round_tf32(v[e][jj].x); v[e][jj].y = cd_round_tf32(v[e][jj].y); }
+        }
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) *reinterpret_cast<float2*>(so + soff(e, jj)) = v[e][jj];
+      }
+      fence_proxy_async();                                 // the staging writes precede the bulk stores' reads
+      wg_sync();
+      if (storer) {
+        tma_store_4d(&mapO, smem_u32(so), co0 + 32 * c, x0, yw, n);
+        if (p.out2) tma_store_4d(&mapO2, smem_u32(so2), co0 + 32 * c, x0, yw, n);
+        bulk_commit();
+      }
+    }
+  }
+  if (storer) bulk_wait<0>();
+}
+
+// ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
 
@@ -416,6 +634,20 @@ template <int BN, int ABOXES, int STAGES, int CTAS = 1>
 int launch_rows(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
   constexpr size_t smem = size_t(ABOXES) * kRowsBoxBytes + size_t(STAGES) * BN * 128 + 1024 + 256;
   return launch_persistent<conv_rows_kernel<BN, ABOXES, STAGES, CTAS>, smem, CTAS>(maps, p, st);
+}
+
+// maps: A0, A1, B0, B1, out, out2 (one CTA per SM)
+template <int BN, int ABOXES, int STAGES>
+int launch_rows256(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
+  constexpr size_t smem = size_t(ABOXES) * kR256BoxBytes + size_t(STAGES) * BN * 128 + 4 * kR256Slice + 1024 + 256;
+  static_assert(smem <= 232448, "dynamic shared memory of one CTA (227 KB)");
+  constexpr auto kernel = conv_rows256_kernel<BN, ABOXES, STAGES>;
+  CD_CUDA(smem_limit_once<kernel>(smem));
+  const int sms = cd_num_sms();
+  const int grid = p.total_tiles < sms ? p.total_tiles : sms;
+  kernel<<<grid, kR256Threads, smem, st>>>(maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], p);
+  CD_LAUNCH_CHECK();
+  return 0;
 }
 
 // Operand conditions of both kernels: nsrc, 16-byte aligned operands, source channels in whole chunks of chunk_elems and a tap
@@ -465,15 +697,16 @@ extern "C" int cd_conv_tc_set_tf32_maps(int enable) { g_tf32_map_dtype = enable 
 // SM for the 64- and 128-wide N tiles (375 -> 387 images/s); the SM-pair kernel took 87 ms.  The shared-row kernel cuts the
 // modelled L2 -> SM bytes of the 3x3 layers 1.2-1.6x; what gains most, though, is that its 128-wide N tiles fit two CTAs per SM
 // for the layers with Cout >= 256 too (a CTA's epilogue then overlaps the other's mainloop): 20-48 % faster on those layers
-// than the per-tap kernel's 256-wide tiles, 0-10 % on the narrower ones.  16 x 16 pixel tiles (two accumulators per weight tile, one CTA per SM) were slower on every layer.
+// than the per-tap kernel's 256-wide tiles, 0-10 % on the narrower ones.  16 x 16 pixel tiles (conv_rows256_kernel, one CTA per SM) are faster still wherever they fill most of a wave (see conv_fwd_rows).
 // A single wave of tiles (16^2, Cout = 256) stays per-tap, and two CTAs per SM are used only with more than one wave of tiles.
 static int g_use_2cta = 0;
 extern "C" int cd_conv_tc_set_2cta(int mode) { g_use_2cta = mode; return 0; }   // 0 off, 1 where the cost model prefers it, 2 wherever eligible
 // narrower pair tiles: bit mask of the N tiles below 256 (128 | 64) that go to the SM-pair kernel when the problem is eligible
 static int g_2cta_bn = 0;
 extern "C" int cd_conv_tc_set_2cta_bn(int mask) { g_2cta_bn = mask & (128 | 64); return 0; }
-// kernel for stride-1 convolutions with taps in [-1, 1]^2: 0 = shape-based choice between the shared-row and the per-tap kernel
-// (default), 1, 2 or 6 = shared-row kernel wherever eligible, 8 = per-tap kernel everywhere
+// kernel for stride-1 convolutions with taps in [-1, 1]^2: 0 = shape-based choice between the shared-row kernels and the per-tap
+// kernel (default), 1, 2 or 6 = shared-row kernel with 16 x 8 tiles wherever eligible, 4 = shared-row kernel with 16 x 16 tiles
+// wherever eligible, 8 = per-tap kernel everywhere
 static int g_use_halo = 0;
 extern "C" int cd_conv_tc_set_halo(int enable) { g_use_halo = enable; return 0; }
 // two CTAs per SM (half the stages each) for N <= 128: bit mask of N tiles (128 | 64)
@@ -509,13 +742,13 @@ extern "C" int cd_conv_fwd_f16_probe(const CdConvDesc* d, void* stream) {
   return conv_fwd_tc_impl(d, static_cast<cudaStream_t>(stream), true);
 }
 
-static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, bool by_shape);
+static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, int mode);
 
 static int conv_fwd_tc_impl(const CdConvDesc* d, cudaStream_t st, bool f16) {
   if (!f16 && g_epi_staged == 0) {
-    // shared-row kernel: chosen by shape (0; the SM-pair switch keeps the per-tap family) or wherever eligible (1, 2, 6)
-    if ((g_use_halo == 0 && !g_use_2cta) || g_use_halo == 1 || g_use_halo == 2 || g_use_halo == 6) {
-      const int r = conv_fwd_rows(d, st, g_use_halo == 0);
+    // shared-row kernels: chosen by shape (0; the SM-pair switch keeps the per-tap family) or wherever eligible (1, 2, 4, 6)
+    if ((g_use_halo == 0 && !g_use_2cta) || g_use_halo == 1 || g_use_halo == 2 || g_use_halo == 4 || g_use_halo == 6) {
+      const int r = conv_fwd_rows(d, st, g_use_halo);
       if (r <= 0) return r;                                   // 1 = not eligible
     }
   }
@@ -594,8 +827,10 @@ static int conv_fwd_tc_impl(const CdConvDesc* d, cudaStream_t st, bool f16) {
 
 // returns 1 when the problem is not eligible for the shared-row kernel -- it needs stride 1, taps in [-1, 1]^2 and a first source
 // whose tap columns hold three taps each on average (dense 3x3; 1x1 and transposed-convolution parity tap lists stay per-tap) --
-// or, with by_shape, when the per-tap kernel is the faster one for this shape (see the measurement above g_use_2cta)
-static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, bool by_shape) {
+// or, in mode 0 (shape-based choice), when the per-tap kernel is the faster one for this shape (see the measurement above
+// g_use_2cta).  Mode 4 takes the 16 x 16 tiles wherever they are eligible, modes 1, 2 and 6 the 16 x 8 tiles.
+static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, int mode) {
+  const bool by_shape = mode == 0;
   if (d->sy != 1 || d->sx != 1 || !operands_ok(d, kChunkK, 4, false)) return 1;
   for (int s = 0; s < d->nsrc; ++s) {
     const CdConvSrc& cs = d->s[s];
@@ -615,8 +850,19 @@ static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, bool by_shape) {
   // per-tap kernel)
   const int sms = cd_num_sms();
   if (by_shape && p.total_tiles <= sms) return 1;
+  // 16 x 16 tiles: the output is stored by TMA through a map over the grid itself (no output pixel map), so the grid must be the
+  // output.  By shape with at least three quarters of a wave of 256-pixel tiles: measured with tools/conv_shapes.py on an H100 80GB
+  // HBM3 at a 700 W power limit (1980 MHz, Unet config 3, batch 32), the 16 x 16 kernel is 4-54 % faster than the 16 x 8 kernel at
+  // two CTAs per SM on every 3x3 forward and data-gradient layer with 128 or more such tiles (e.g. 393 against 804 us for 128^2,
+  // Cout = 128, K = 576; 993 against 1154 us for its data gradient) but for one (+5 %, 16^2 data gradient, Cout = 512, K = 2304),
+  // and 17-36 % slower with 64 tiles (16^2, Cout = 256), which stay on the per-tap kernel anyway.  The 3x3 forward + data-gradient
+  // convolutions of one micro-batch take 23.5 ms instead of 27.2 ms.
+  const int tiles256 = p.tiles_x * cd_cdiv(d->Hg, kR256TH) * p.tiles_n * p.tiles_co;
+  const bool rows256 = (mode == 4 || (by_shape && 4 * tiles256 >= 3 * sms)) && d->oys == 1 && d->oxs == 1 && d->oy0 == 0 &&
+                       d->ox0 == 0 && d->Ho == d->Hg && d->Wo == d->Wg;
+  if (rows256) { p.TH = kR256TH; p.tiles_y = cd_cdiv(d->Hg, kR256TH); p.total_tiles = tiles256; }
   const CUtensorMapDataType dt = g_tf32_map_dtype ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  CUtensorMap maps[4];
+  CUtensorMap maps[6];
   for (int s = 0; s < 2; ++s) {
     const CdConvSrc& cs = d->s[s < d->nsrc ? s : 0];
     int i = 0;
@@ -627,11 +873,24 @@ static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, bool by_shape) {
       if (i > i0) { p.boxdx[s][p.nbox[s]] = (int8_t)dx; p.boxend[s][p.nbox[s]] = (int8_t)i; ++p.nbox[s]; }
     }
     if (s == 0 && cs.ntaps < 3 * p.nbox[0]) return 1;
-    // A: one box {32 ch, 16, 8 + 2, 1} per chunk and tap column
-    if (!encode_nhwc(&maps[s], dt, cs.src, cs.ld, cs.C, cs.W, cs.H, d->B, 1, 1, 0, 0, kRowsTW, kRowsTH + 2, 1, 1, 1,
+    // A: one box {32 ch, 16, TH + 2, 1} per chunk and tap column
+    if (!encode_nhwc(&maps[s], dt, cs.src, cs.ld, cs.C, cs.W, cs.H, d->B, 1, 1, 0, 0, kRowsTW, p.TH + 2, 1, 1, 1,
                      s ? "rows A1" : "rows A0") ||
         !encode_weights(&maps[2 + s], dt, cs.w, cs.C, d->Cout, cs.ntaps, BN, s ? "rows B1" : "rows B0"))
       return -1;
+  }
+  if (rows256) {
+    // out / out2: one warpgroup's box {32 ch, 16, 8, 1} per store, fp32 bits as computed
+    const float* o2 = d->out2 ? d->out2 : d->out;
+    const int o2ld = d->out2 ? d->out2_ld : d->out_ld;
+    if (!encode_nhwc(&maps[4], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, d->out, d->out_ld, d->Cout, d->Wg, d->Hg, d->B, 1, 1, 0, 0, kRowsTW,
+                     kR256TH / 2, 1, 1, 1, "rows out") ||
+        !encode_nhwc(&maps[5], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, o2, o2ld, d->Cout, d->Wg, d->Hg, d->B, 1, 1, 0, 0, kRowsTW,
+                     kR256TH / 2, 1, 1, 1, "rows out2"))
+      return -1;
+    // three boxes (108 KB), 48 KB of weight tiles and 64 KB of staging slices
+    if (BN == 128) return launch_rows256<128, 3, 3>(maps, p, st);
+    return launch_rows256<64, 3, 6>(maps, p, st);
   }
   // one CTA per SM: six boxes (120 KB) and 64 KB of weight tiles; two CTAs per SM: three boxes and 48 KB of weight tiles each
   const int ctas2 = p.total_tiles > sms ? g_ctas2 : 0;

@@ -17,7 +17,6 @@ constexpr int kWTX = 16;           // weight gradient: output columns per tile
 __device__ __forceinline__ float* align128(uint8_t* raw) {      // bulk tensor copies need a 128-byte aligned destination
   return reinterpret_cast<float*>(raw + ((128u - (smem_u32(raw) & 127u)) & 127u));
 }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 template <int TX>
 __global__ void __launch_bounds__(32 * kTY, 1)

@@ -57,6 +57,21 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       :: "r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)),
          "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
+// orders this thread's generic-proxy shared-memory accesses before later async-proxy (TMA, wgmma) accesses of the same bytes
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// shared -> global tensor store of one 4-D box (coordinates as tma_load_4d; out-of-bounds elements of the box are not written),
+// tracked by the issuing thread's bulk async-groups
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               :: "l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" :: "n"(N) : "memory"); }
+// at most N of this thread's committed bulk groups are still incomplete (their global writes included)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" :: "n"(N) : "memory"); }
 // K-major SWIZZLE_128B operand descriptor of wgmma: rows of 128 bytes, 8-row groups 1024 bytes apart.  Advancing the start
 // address by 32 bytes selects the next K step inside the swizzle row (the swizzle is applied to the final address bits).
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t saddr) {

@@ -216,8 +216,8 @@ int cd_conv_tc_set_2cta_bn(int mask);
 /* kernel choice for stride-1 convolutions whose taps lie in [-1, 1]^2 (dense 3x3 forward / data gradient, fused [3x3 | 1x1]
  * pairs).  The shared-row kernel fetches one TW x (TH + 2) activation box per 32-channel chunk and tap column and feeds the three
  * row taps of that column from it; the per-tap kernel fetches one 128-pixel box per tap.  0 = shape-based choice (default),
- * 1, 2 or 6 = shared-row kernel with 16 x 8 pixel tiles wherever eligible, 3 = shared-row kernel with 8 x 16 tiles wherever
- * eligible, 8 = per-tap kernel everywhere.  With the SM-pair kernel on (cd_conv_tc_set_2cta), 0 keeps the per-tap family. */
+ * 1, 2 or 6 = shared-row kernel with 16 x 8 pixel tiles wherever eligible, 4 = shared-row kernel with 16 x 16 pixel tiles (one
+ * CTA per SM, output stored by TMA) wherever eligible and the output map is the identity, 8 = per-tap kernel everywhere.  With the SM-pair kernel on (cd_conv_tc_set_2cta), 0 keeps the per-tap family. */
 int cd_conv_tc_set_halo(int enable);
 /* two co-resident CTAs per SM (half the pipeline stages each) for the tensor-core convolution with N <= 128: one CTA's epilogue
  * overlaps the other's mainloop.  Bit mask of N tiles (128 | 64); default 192 (both), 0 = one CTA per SM */
