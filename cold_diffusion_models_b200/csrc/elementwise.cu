@@ -783,51 +783,28 @@ extern "C" int cd_nchw_to_nhwc(const float* x, int B, int C, int H, int W, float
 // transpose (value matrix of the AttnBlock, M2:178-181) and NHWC -> NCHW for the 3-channel output.
 // =============================================================================================================
 namespace {
-// one block per batch element: pass 1 accumulates per-group sum / sum of squares (fp32), pass 2 normalises.
+// one block per batch element: (mean, rstd) per group from cd_gn_plane_stats (cd_common.cuh: shifted per-thread sums merged
+// with Chan's formula in a fixed order), then y = (x + cond - mean) * rstd * gamma + beta [swish].
 __global__ void __launch_bounds__(512)
 groupnorm_kernel(const float* __restrict__ x, int x_ld, int HW, int C, int groups, const float* __restrict__ cond, int cond_ld,
                  const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int swish,
                  float* __restrict__ y, int y_ld) {
-  extern __shared__ float sm[];                 // sum[groups] | sq[groups] | part[8][blockDim]
-  float* gsum = sm; float* gsq = sm + groups; float* part = sm + 2 * groups;
+  __shared__ float tm[4][512], tq[4][512];
+  extern __shared__ float gst[];                // (mean, rstd)[groups]
   const int b = blockIdx.x;
   const int nq = C >> 2, cg = C / groups;
   const long long base = static_cast<long long>(b) * HW;
   // thread -> (pixel lane, channel quad): consecutive threads walk consecutive quads of one pixel (coalesced)
   const int q = threadIdx.x % nq, pl = threadIdx.x / nq, np = blockDim.x / nq;
-  float4 cadd = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (cond && pl < np) cadd = *reinterpret_cast<const float4*>(cond + static_cast<long long>(b) * cond_ld + q * 4);
-  if (pl < np) {
-    float s[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-    for (int p = pl; p < HW; p += np) {
-      float4 v = *reinterpret_cast<const float4*>(x + (base + p) * x_ld + q * 4);
-      v.x += cadd.x; v.y += cadd.y; v.z += cadd.z; v.w += cadd.w;
-      s[0] += v.x; s[1] += v.y; s[2] += v.z; s[3] += v.w;
-      s2[0] += v.x * v.x; s2[1] += v.y * v.y; s2[2] += v.z * v.z; s2[3] += v.w * v.w;
-    }
-    // per-thread partial sums go to shared memory and are added per group in a FIXED order below (shared-memory atomics made the
-    // statistics, and through the TF32 roundings downstream the network output, differ from run to run)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) { part[j * blockDim.x + threadIdx.x] = s[j]; part[(4 + j) * blockDim.x + threadIdx.x] = s2[j]; }
-  }
+  cd_gn_plane_stats(x, x_ld, HW, C, groups, cond, cond_ld, eps, b, tm, tq, gst);
   __syncthreads();
-  for (int g = threadIdx.x; g < groups; g += blockDim.x) {
-    float a = 0.f, a2 = 0.f;
-    for (int c = g * cg; c < (g + 1) * cg; ++c) {
-      const int qq = c >> 2, j = c & 3;
-      for (int pp = 0; pp < np; ++pp) { a += part[j * blockDim.x + pp * nq + qq]; a2 += part[(4 + j) * blockDim.x + pp * nq + qq]; }
-    }
-    gsum[g] = a; gsq[g] = a2;
-  }
-  __syncthreads();
-  const float inv_n = 1.f / (static_cast<float>(HW) * cg);
   if (pl < np) {
+    float4 cadd = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (cond) cadd = *reinterpret_cast<const float4*>(cond + static_cast<long long>(b) * cond_ld + q * 4);
     float mean[4], rstd[4];
     for (int j = 0; j < 4; ++j) {
       const int g = (q * 4 + j) / cg;
-      mean[j] = gsum[g] * inv_n;
-      const float var = fmaxf(gsq[g] * inv_n - mean[j] * mean[j], 0.f);
-      rstd[j] = rsqrtf(var + eps);
+      mean[j] = gst[2 * g]; rstd[j] = gst[2 * g + 1];
     }
     const float4 gm = *reinterpret_cast<const float4*>(gamma + q * 4);
     const float4 bt = *reinterpret_cast<const float4*>(beta + q * 4);
@@ -962,70 +939,17 @@ time_mlp2_dense_kernel(const long long* __restrict__ t, int dim, int hid, int td
 // (pixel lane, channel quad) mapping of groupnorm_kernel; chunk k of image b covers pixels [k * cp, (k + 1) * cp), cp =
 // cd_gn_split_chunk(C) = GN_SPLIT_ITERS pixels per active thread.  Statistics are (count, mean, M2) triples merged with Chan's
 // formula in a fixed order (no E[x^2] - mean^2 cancellation for inputs with a large mean, no float atomics).
-// merge (nb, meanb, m2b) into (n, mean, m2)
-__device__ __forceinline__ void chan_merge(float& n, float& mean, float& m2, float nb, float meanb, float m2b) {
-  if (nb == 0.f) return;
-  const float nn = n + nb, d = meanb - mean;
-  mean += d * (nb / nn);
-  m2 += m2b + d * d * (n * nb / nn);
-  n = nn;
-}
-
-// fixed-order tree over the lanes of a warp; lane 0 ends with the merge of all 32
-__device__ __forceinline__ void chan_warp_merge(float& n, float& mean, float& m2) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float nb = __shfl_down_sync(0xffffffffu, n, o), mb = __shfl_down_sync(0xffffffffu, mean, o);
-    const float qb = __shfl_down_sync(0xffffffffu, m2, o);
-    if ((threadIdx.x & 31) + o < 32 && ((threadIdx.x & 31) & (2 * o - 1)) == 0) chan_merge(n, mean, m2, nb, mb, qb);
-  }
-}
-
-// pass 1: per-(image, chunk, group) (mean, M2) of x + cond -> part[b][k][g][2]; the count is implied by the chunk geometry.
-// Each thread keeps shifted sums about its first value (one chunk holds at most GN_SPLIT_ITERS values per thread-channel),
-// then one warp per group merges the thread-channel triples.
+// pass 1: per-(image, chunk, group) (mean, M2) of x + cond -> part[b][k][g][2] (cd_gn_chunk_stats); the count is implied by
+// the chunk geometry
 __global__ void __launch_bounds__(512)
 gn_split_stats_kernel(const float* __restrict__ x, int x_ld, long long HW, int C, int groups, const float* __restrict__ cond,
                       int cond_ld, int cp, float* __restrict__ part) {
   __shared__ float tm[4][512], tq[4][512];
   const int k = blockIdx.x, b = blockIdx.y, nch = gridDim.x;
-  const int nq = C >> 2, cg = C / groups;
-  const int q = threadIdx.x % nq, pl = threadIdx.x / nq, np = blockDim.x / nq;
-  const long long base = static_cast<long long>(b) * HW + static_cast<long long>(k) * cp;
-  if (pl < np) {
-    float4 cadd = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (cond) cadd = *reinterpret_cast<const float4*>(cond + static_cast<long long>(b) * cond_ld + q * 4);
-    const int cnt = cd_gn_lane_count(HW, k, cp, pl, np);
-    float sh[4] = {0.f, 0.f, 0.f, 0.f}, s[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 4
-    for (int i = 0; i < cnt; ++i) {
-      float4 v = *reinterpret_cast<const float4*>(x + (base + pl + static_cast<long long>(i) * np) * x_ld + q * 4);
-      const float w[4] = {v.x + cadd.x, v.y + cadd.y, v.z + cadd.z, v.w + cadd.w};
-      if (i == 0) for (int j = 0; j < 4; ++j) sh[j] = w[j];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) { const float d = w[j] - sh[j]; s[j] += d; s2[j] += d * d; }
-    }
-    const float inv = cnt > 0 ? 1.f / static_cast<float>(cnt) : 0.f;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      tm[j][threadIdx.x] = sh[j] + s[j] * inv;
-      tq[j][threadIdx.x] = fmaxf(s2[j] - s[j] * s[j] * inv, 0.f);
-    }
-  }
-  __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  for (int g = warp; g < groups; g += nw) {
-    float n = 0.f, mean = 0.f, m2 = 0.f;
-    for (int e = lane; e < cg * np; e += 32) {           // entry e: channel g*cg + e/np of pixel lane e%np
-      const int c = g * cg + e / np, pp = e % np, t = pp * nq + (c >> 2);
-      chan_merge(n, mean, m2, static_cast<float>(cd_gn_lane_count(HW, k, cp, pp, np)), tm[c & 3][t], tq[c & 3][t]);
-    }
-    chan_warp_merge(n, mean, m2);
-    if (lane == 0) {
-      float* o = part + ((static_cast<long long>(b) * nch + k) * groups + g) * 2;
-      o[0] = mean; o[1] = m2;
-    }
-  }
+  cd_gn_chunk_stats(x, x_ld, HW, C, groups, cond, cond_ld, b, k, cp, tm, tq, [&](int g, float, float mean, float m2) {
+    float* o = part + ((static_cast<long long>(b) * nch + k) * groups + g) * 2;
+    o[0] = mean; o[1] = m2;
+  });
 }
 
 // pass 2: merge the chunks of each (image, group) in a fixed order -> stats[b][g] = (mean, rstd); one warp per group
@@ -1038,9 +962,9 @@ gn_split_combine_kernel(const float* __restrict__ part, long long HW, int cg, in
     for (int k = lane; k < nch; k += 32) {
       const float* p = part + ((static_cast<long long>(b) * nch + k) * groups + g) * 2;
       const long long pix = HW - static_cast<long long>(k) * cp < cp ? HW - static_cast<long long>(k) * cp : cp;
-      chan_merge(n, mean, m2, static_cast<float>(pix * cg), p[0], p[1]);
+      cd_chan_merge(n, mean, m2, static_cast<float>(pix * cg), p[0], p[1]);
     }
-    chan_warp_merge(n, mean, m2);
+    cd_chan_warp_merge(n, mean, m2);
     if (lane == 0) {
       stats[(static_cast<long long>(b) * groups + g) * 2] = mean;
       stats[(static_cast<long long>(b) * groups + g) * 2 + 1] = rsqrtf(m2 / n + eps);
@@ -1141,7 +1065,7 @@ extern "C" int cd_groupnorm_fwd(const float* x, int x_ld, int B, int64_t HW, int
     CD_LAUNCH_CHECK();
     return 0;
   }
-  groupnorm_kernel<<<B, 512, sizeof(float) * (2 * groups + 8 * 512), static_cast<cudaStream_t>(stream)>>>(x, x_ld, (int)HW, C, groups, cond, cond_ld,
+  groupnorm_kernel<<<B, 512, sizeof(float) * 2 * groups, static_cast<cudaStream_t>(stream)>>>(x, x_ld, (int)HW, C, groups, cond, cond_ld,
                                                                                            gamma, beta, eps, swish, y, y_ld);
   CD_LAUNCH_CHECK();
   return 0;

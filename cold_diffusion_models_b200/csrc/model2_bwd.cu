@@ -12,49 +12,45 @@ namespace {
 __device__ __forceinline__ float sigmoidf_(float z) { return 1.f / (1.f + __expf(-z)); }
 __device__ __forceinline__ float swish_grad(float z) { const float s = sigmoidf_(z); return s * (1.f + z * (1.f - s)); }
 
+// per-channel sum over the pixel lanes of a CTA in lane order: v[j][pp * nq + c / 4] holds channel c of pixel lane pp
+__device__ __forceinline__ float gn_lane_sum(const float (*v)[512], int c, int nq, int np) {
+  float a = 0.f;
+  for (int pp = 0; pp < np; ++pp) a += v[c & 3][pp * nq + (c >> 2)];
+  return a;
+}
+
 // one block per batch element (same thread -> (pixel lane, channel quad) mapping as groupnorm_kernel in elementwise.cu)
 //   z = gamma * xh + beta, xh = (x + cond - mean_g) * rstd_g, y = swish ? z*sigmoid(z) : z
 //   dz = dy * (swish ? swish'(z) : 1);  dgamma_c += sum dz*xh;  dbeta_c += sum dz
 //   dx = rstd_g * (dz*gamma - mean_g(dz*gamma) - xh * mean_g(dz*gamma*xh));  dcond[b][c] = sum_pixels dx
+// mean_g and rstd_g come from cd_gn_plane_stats, as in the forward (the same bits); every sum within the CTA is added in a fixed
+// order (gn_lane_sum), so the result does not depend on the order the threads run in.
 __global__ void __launch_bounds__(512)
 groupnorm_bwd_kernel(const float* __restrict__ x, int x_ld, int HW, int C, int groups, const float* __restrict__ cond, int cond_ld,
                      const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int swish,
                      const float* __restrict__ dy, int dy_ld, float* __restrict__ dx, int dx_ld,
                      float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dcond, int dcond_ld) {
-  extern __shared__ float sm[];        // gsum[G] | gsq[G] | ga[G] | gb[G] | cdz[C] | cdzx[C] | cdx[C]
-  float* gsum = sm; float* gsq = gsum + groups; float* ga = gsq + groups; float* gb = ga + groups;
-  float* cdz = gb + groups; float* cdzx = cdz + C; float* cdx = cdzx + C;
+  __shared__ float ta[4][512], tb[4][512];   // statistics scratch, then per-thread sums of dz | dz*xh, then of dx
+  extern __shared__ float sm[];               // gst[G][2] (mean, rstd) | gab[G][2] | cdz[C] | cdzx[C]
+  float* gst = sm; float* gab = gst + 2 * groups; float* cdz = gab + 2 * groups; float* cdzx = cdz + C;
   const int b = blockIdx.x;
   const int nq = C >> 2, cg = C / groups;
-  for (int i = threadIdx.x; i < 4 * groups + 3 * C; i += blockDim.x) sm[i] = 0.f;
+  cd_gn_plane_stats(x, x_ld, HW, C, groups, cond, cond_ld, eps, b, ta, tb, gst);
   __syncthreads();
   const long long base = static_cast<long long>(b) * HW;
   const int q = threadIdx.x % nq, pl = threadIdx.x / nq, np = blockDim.x / nq;
   const bool act = pl < np;
   float cadd[4] = {0.f, 0.f, 0.f, 0.f};
   if (cond && act) { const float4 cv = *reinterpret_cast<const float4*>(cond + static_cast<long long>(b) * cond_ld + q * 4); cadd[0] = cv.x; cadd[1] = cv.y; cadd[2] = cv.z; cadd[3] = cv.w; }
-  // ---- pass 1: group statistics
-  if (act) {
-    float s[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-    for (int p = pl; p < HW; p += np) {
-      const float4 v4 = *reinterpret_cast<const float4*>(x + (base + p) * x_ld + q * 4);
-      const float v[4] = {v4.x + cadd[0], v4.y + cadd[1], v4.z + cadd[2], v4.w + cadd[3]};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) { s[j] += v[j]; s2[j] += v[j] * v[j]; }
-    }
-    for (int j = 0; j < 4; ++j) { atomicAdd(&gsum[(q * 4 + j) / cg], s[j]); atomicAdd(&gsq[(q * 4 + j) / cg], s2[j]); }
-  }
-  __syncthreads();
   const float inv_n = 1.f / (static_cast<float>(HW) * cg);
   float mean[4], rstd[4], gm[4] = {0.f, 0.f, 0.f, 0.f}, bt[4] = {0.f, 0.f, 0.f, 0.f};
   if (act) {
     for (int j = 0; j < 4; ++j) {
       const int g = (q * 4 + j) / cg;
-      mean[j] = gsum[g] * inv_n;
-      rstd[j] = rsqrtf(fmaxf(gsq[g] * inv_n - mean[j] * mean[j], 0.f) + eps);
+      mean[j] = gst[2 * g]; rstd[j] = gst[2 * g + 1];
       gm[j] = gamma[q * 4 + j]; bt[j] = beta[q * 4 + j];
     }
-    // ---- pass 2: per-channel sums of dz and dz*xh
+    // ---- per-channel sums of dz and dz*xh
     float sdz[4] = {0.f, 0.f, 0.f, 0.f}, sdzx[4] = {0.f, 0.f, 0.f, 0.f};
     for (int p = pl; p < HW; p += np) {
       const float4 v4 = *reinterpret_cast<const float4*>(x + (base + p) * x_ld + q * 4);
@@ -68,21 +64,25 @@ groupnorm_bwd_kernel(const float* __restrict__ x, int x_ld, int HW, int C, int g
         sdz[j] += dz; sdzx[j] += dz * xh;
       }
     }
-    for (int j = 0; j < 4; ++j) { atomicAdd(&cdz[q * 4 + j], sdz[j]); atomicAdd(&cdzx[q * 4 + j], sdzx[j]); }
+    for (int j = 0; j < 4; ++j) { ta[j][threadIdx.x] = sdz[j]; tb[j][threadIdx.x] = sdzx[j]; }
   }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    cdz[c] = gn_lane_sum(ta, c, nq, np); cdzx[c] = gn_lane_sum(tb, c, nq, np);
     atomicAdd(dgamma + c, cdzx[c]);
     atomicAdd(dbeta + c, cdz[c]);
-    const float gc = gamma[c];
-    atomicAdd(&ga[c / cg], gc * cdz[c]);
-    atomicAdd(&gb[c / cg], gc * cdzx[c]);
   }
   __syncthreads();
-  // ---- pass 3: dx (+ per-channel sums for the conditioning gradient)
+  for (int g = threadIdx.x; g < groups; g += blockDim.x) {
+    float a = 0.f, a2 = 0.f;
+    for (int c = g * cg; c < (g + 1) * cg; ++c) { a += gamma[c] * cdz[c]; a2 += gamma[c] * cdzx[c]; }
+    gab[2 * g] = a * inv_n; gab[2 * g + 1] = a2 * inv_n;
+  }
+  __syncthreads();
+  // ---- dx (+ per-channel sums for the conditioning gradient)
   if (act) {
     float ma[4], mb[4], sdx[4] = {0.f, 0.f, 0.f, 0.f};
-    for (int j = 0; j < 4; ++j) { const int g = (q * 4 + j) / cg; ma[j] = ga[g] * inv_n; mb[j] = gb[g] * inv_n; }
+    for (int j = 0; j < 4; ++j) { const int g = (q * 4 + j) / cg; ma[j] = gab[2 * g]; mb[j] = gab[2 * g + 1]; }
     for (int p = pl; p < HW; p += np) {
       const float4 v4 = *reinterpret_cast<const float4*>(x + (base + p) * x_ld + q * 4);
       const float4 d4 = *reinterpret_cast<const float4*>(dy + (base + p) * dy_ld + q * 4);
@@ -98,24 +98,17 @@ groupnorm_bwd_kernel(const float* __restrict__ x, int x_ld, int HW, int C, int g
       }
       *reinterpret_cast<float4*>(dx + (base + p) * dx_ld + q * 4) = make_float4(o[0], o[1], o[2], o[3]);
     }
-    if (dcond) for (int j = 0; j < 4; ++j) atomicAdd(&cdx[q * 4 + j], sdx[j]);
+    for (int j = 0; j < 4; ++j) ta[j][threadIdx.x] = sdx[j];
   }
   if (dcond) {
     __syncthreads();
-    for (int c = threadIdx.x; c < C; c += blockDim.x) dcond[static_cast<long long>(b) * dcond_ld + c] = cdx[c];
+    for (int c = threadIdx.x; c < C; c += blockDim.x) dcond[static_cast<long long>(b) * dcond_ld + c] = gn_lane_sum(ta, c, nq, np);
   }
 }
 
 // ---- split-plane backward (planes above CD_GN_SPLIT_MIN_HW pixels; the (chunk x image) grid and thread mapping of the
 // forward's gn_split_* kernels in elementwise.cu).  Every per-channel sum is formed per chunk and the chunks are added in a
 // fixed order: no float atomics, run-to-run identical results.
-// per-channel sum over the pixel lanes of a CTA in lane order: v[j][pp * nq + c / 4] holds channel c of pixel lane pp
-__device__ __forceinline__ float gn_lane_sum(const float (*v)[512], int c, int nq, int np) {
-  float a = 0.f;
-  for (int pp = 0; pp < np; ++pp) a += v[c & 3][pp * nq + (c >> 2)];
-  return a;
-}
-
 // out[c] = sum over k < nch of src[k * stride + c] in a fixed order: slice s of nsl = max(1, blockDim / C) adds k = s, s + nsl,
 // ..., then the slices are added in order.  scratch holds nsl * C <= 2048 floats.
 __device__ void gn_chunk_colsum(const float* __restrict__ src, long long stride, int nch, int C, float* scratch, float* out) {
@@ -403,7 +396,14 @@ extern "C" int cd_groupnorm_bwd(const float* x, int x_ld, int B, int64_t HW, int
     CD_LAUNCH_CHECK();
     return 0;
   }
-  const size_t smem = sizeof(float) * (4 * groups + 3 * C);
+  // dynamic shared memory beyond 48 KB less the kernel's 16 KB of static scratch (4 * groups + 2 * C > 8192, e.g. groups == C
+  // above 1365) needs the opt-in; at most 48 KB + 16 KB
+  const size_t smem = sizeof(float) * (4 * groups + 2 * C);
+  static size_t attr = 0;
+  if (smem > 32 * 1024 && smem > attr) {
+    CD_CUDA(cudaFuncSetAttribute(groupnorm_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr = smem;
+  }
   groupnorm_bwd_kernel<<<B, 512, smem, static_cast<cudaStream_t>(stream)>>>(x, x_ld, (int)HW, C, groups, cond, cond_ld, gamma, beta, eps, swish,
                                                                          dy, dy_ld, dx, dx_ld, dgamma, dbeta, dcond, dcond_ld);
   CD_LAUNCH_CHECK();

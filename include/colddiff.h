@@ -339,10 +339,12 @@ int cd_snow_layers(const double* noise, int SB, int ch, int m, int trim, int H, 
  * convolutions (3x3, 1x1 q/k/v/proj/nin_shortcut, asymmetric-pad stride-2 Downsample, and the two batched matmuls of AttnBlock
  * as per-batch-weight 1x1 tap-list convolutions) run through cd_conv_fwd.
  * ------------------------------------------------------------------------------------------ */
-/* GroupNorm(groups, eps) of (x + cond[b,c]) [* swish] on NHWC (M2:32-33, 114-123).  HW <= 128*128: one CTA per image.
- * Larger planes: a (pixel chunk x image) grid with Chan-merged statistics and fixed-order sums (cd_groupnorm_bwd too); its
- * partials go to a device buffer cached per (device, stream) that grows outside CUDA-graph capture only (a capture that
- * would need it larger fails: run the shape once before capturing).  Needs C % 4 == 0, C / 4 <= 512 and B <= 65535. */
+/* GroupNorm(groups, eps) of (x + cond[b,c]) [* swish] on NHWC (M2:32-33, 114-123).  Statistics are Chan-merged (count,
+ * mean, M2) triples and every sum within an image is added in a fixed order (cd_groupnorm_bwd too): accurate for inputs
+ * with a large mean, and the same bits run to run (except dgamma / dbeta on planes of at most 128*128 pixels, to which the
+ * images add atomically).  HW <= 128*128: one CTA per image.  Larger planes: a (pixel chunk x image) grid; its partials go to
+ * a device buffer cached per (device, stream) that grows outside CUDA-graph capture only (a capture that would need it larger
+ * fails: run the shape once before capturing).  Needs C % 4 == 0, C / 4 <= 512 and B <= 65535. */
 int cd_groupnorm_fwd(const float* x, int x_ld, int B, int64_t HW, int C, int groups, const float* cond, int cond_ld,
                      const float* gamma, const float* beta, float eps, int swish, float* y, int y_ld, void* stream);
 /* in-place softmax(scale * s) over the last dimension of [rows][n] (M2:172-175) */

@@ -84,15 +84,15 @@ def _grad_check(ck, name, eg, ref, ctrl, bmed, bworst):
 # ==========================================================================================================================
 # the GroupNorm entry points on 256² planes
 # ==========================================================================================================================
-def _gn64(x, cond, gamma, beta, swish, B, HW, Cc):
+def _gn64(x, cond, gamma, beta, swish, B, HW, Cc, groups=32):
     h = (x.to(F64).view(B, HW, Cc) + cond.to(F64)[:, None, :]).permute(0, 2, 1)
-    z = F.group_norm(h, 32, gamma.to(F64), beta.to(F64), eps=1e-6).permute(0, 2, 1)
+    z = F.group_norm(h, groups, gamma.to(F64), beta.to(F64), eps=1e-6).permute(0, 2, 1)
     return z * torch.sigmoid(z) if swish else z
 
 
-def _fp32_one_pass(x, cond, gamma, beta, B, HW, Cc):
+def _fp32_one_pass(x, cond, gamma, beta, B, HW, Cc, groups=32):
     """the one-pass fp32 statistics E[v^2] - mean^2 (the negative control of the large-mean case)"""
-    v = x.view(B, HW, 32, Cc // 32) + cond.view(B, 1, 32, Cc // 32)
+    v = x.view(B, HW, groups, Cc // groups) + cond.view(B, 1, groups, Cc // groups)
     mean = v.mean(dim=(1, 3), keepdim=True)
     var = ((v * v).mean(dim=(1, 3), keepdim=True) - mean * mean).clamp_min(0)
     z = ((v - mean) * torch.rsqrt(var + 1e-6)).view(B, HW, Cc) * gamma + beta

@@ -38,14 +38,14 @@ NET = dict(ch=128, ch_mult=(1, 2, 2, 2), num_res_blocks=2, attn_resolutions=(16,
 _PROBE = {'elementwise.cu': r'''
 extern "C" int probe_gn_fwd(const float* x, int x_ld, int B, int HW, int C, int groups, const float* cond, int cond_ld,
                             const float* gamma, const float* beta, float eps, int swish, float* y, int y_ld, void* st) {
-  groupnorm_kernel<<<B, 512, sizeof(float) * (2 * groups + 8 * 512), static_cast<cudaStream_t>(st)>>>(x, x_ld, HW, C, groups, cond,
+  groupnorm_kernel<<<B, 512, sizeof(float) * 2 * groups, static_cast<cudaStream_t>(st)>>>(x, x_ld, HW, C, groups, cond,
       cond_ld, gamma, beta, eps, swish, y, y_ld);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }''', 'model2_bwd.cu': r'''
 extern "C" int probe_gn_bwd(const float* x, int x_ld, int B, int HW, int C, int groups, const float* cond, int cond_ld,
                             const float* gamma, const float* beta, float eps, int swish, const float* dy, int dy_ld, float* dx,
                             int dx_ld, float* dgamma, float* dbeta, float* dcond, int dcond_ld, void* st) {
-  groupnorm_bwd_kernel<<<B, 512, sizeof(float) * (4 * groups + 3 * C), static_cast<cudaStream_t>(st)>>>(x, x_ld, HW, C, groups,
+  groupnorm_bwd_kernel<<<B, 512, sizeof(float) * (4 * groups + 2 * C), static_cast<cudaStream_t>(st)>>>(x, x_ld, HW, C, groups,
       cond, cond_ld, gamma, beta, eps, swish, dy, dy_ld, dx, dx_ld, dgamma, dbeta, dcond, dcond_ld);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }'''}
