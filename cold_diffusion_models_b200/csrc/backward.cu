@@ -12,7 +12,8 @@ namespace {
 // ---------------------------------------------------------------------------------------------
 // lanes are split into groups of G = min(32, C/4) (a power of two): each group owns one pixel per iteration, each lane
 // C/(4G) float4 slots; two iterations are in flight per warp so the load->reduce->store chain is not latency-bound.
-template <int NQ, int PP>     // float4 slots per lane, pixel groups per trip
+// kParams = false (dg = dbeta = NULL, frozen g and b): dh only, the parameter sums and their block reduction are compiled out.
+template <int NQ, int PP, bool kParams>     // float4 slots per lane, pixel groups per trip, parameter gradients
 __global__ void __launch_bounds__(256, NQ == 1 ? 3 : 1)
 layernorm_bwd_kernel(const float* __restrict__ dy, int dy_ld, const float* __restrict__ h, int h_ld,
                      const float* __restrict__ stats, const float* __restrict__ g, long long npix, int C,
@@ -71,8 +72,10 @@ layernorm_bwd_kernel(const float* __restrict__ dy, int dy_ld, const float* __res
           const float4 d = dl[k][i];
           const float4 hv = hl[k][i];
           xh[i] = make_float4((hv.x - mean[k]) * rstd[k], (hv.y - mean[k]) * rstd[k], (hv.z - mean[k]) * rstd[k], (hv.w - mean[k]) * rstd[k]);
-          ag[i].x += d.x * xh[i].x; ag[i].y += d.y * xh[i].y; ag[i].z += d.z * xh[i].z; ag[i].w += d.w * xh[i].w;
-          ab[i].x += d.x; ab[i].y += d.y; ab[i].z += d.z; ab[i].w += d.w;
+          if constexpr (kParams) {
+            ag[i].x += d.x * xh[i].x; ag[i].y += d.y * xh[i].y; ag[i].z += d.z * xh[i].z; ag[i].w += d.w * xh[i].w;
+            ab[i].x += d.x; ab[i].y += d.y; ab[i].z += d.z; ab[i].w += d.w;
+          }
           dv[i] = make_float4(d.x * gv[i].x, d.y * gv[i].y, d.z * gv[i].z, d.w * gv[i].w);
           s1 += dv[i].x + dv[i].y + dv[i].z + dv[i].w;
           s2 += dv[i].x * xh[i].x + dv[i].y * xh[i].y + dv[i].z * xh[i].z + dv[i].w * xh[i].w;
@@ -96,21 +99,23 @@ layernorm_bwd_kernel(const float* __restrict__ dy, int dy_ld, const float* __res
       }
     }
   }
-  // block reduction of the parameter gradients, one atomicAdd per channel per block
-  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) red[i] = 0.f;
-  __syncthreads();
+  if constexpr (kParams) {
+    // block reduction of the parameter gradients, one atomicAdd per channel per block
+    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) red[i] = 0.f;
+    __syncthreads();
 #pragma unroll
-  for (int i = 0; i < NQ; ++i) {
-    const int qd = gl + i * G;
-    if (qd < nq) {
-      atomicAdd(&red[qd * 4 + 0], ag[i].x); atomicAdd(&red[qd * 4 + 1], ag[i].y);
-      atomicAdd(&red[qd * 4 + 2], ag[i].z); atomicAdd(&red[qd * 4 + 3], ag[i].w);
-      atomicAdd(&red[C + qd * 4 + 0], ab[i].x); atomicAdd(&red[C + qd * 4 + 1], ab[i].y);
-      atomicAdd(&red[C + qd * 4 + 2], ab[i].z); atomicAdd(&red[C + qd * 4 + 3], ab[i].w);
+    for (int i = 0; i < NQ; ++i) {
+      const int qd = gl + i * G;
+      if (qd < nq) {
+        atomicAdd(&red[qd * 4 + 0], ag[i].x); atomicAdd(&red[qd * 4 + 1], ag[i].y);
+        atomicAdd(&red[qd * 4 + 2], ag[i].z); atomicAdd(&red[qd * 4 + 3], ag[i].w);
+        atomicAdd(&red[C + qd * 4 + 0], ab[i].x); atomicAdd(&red[C + qd * 4 + 1], ab[i].y);
+        atomicAdd(&red[C + qd * 4 + 2], ab[i].z); atomicAdd(&red[C + qd * 4 + 3], ab[i].w);
+      }
     }
+    __syncthreads();
+    for (int i = threadIdx.x; i < C; i += blockDim.x) { atomicAdd(dg + i, red[i]); atomicAdd(dbeta + i, red[C + i]); }
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < C; i += blockDim.x) { atomicAdd(dg + i, red[i]); atomicAdd(dbeta + i, red[C + i]); }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -570,9 +575,13 @@ extern "C" int cd_layernorm_bwd(const float* dy, int dy_ld, const float* h, int 
   if (ppb < 32) ppb = 32;
   const int blocks = cd_cdiv(npix, ppb);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t smem = sizeof(float) * 2 * C;
+  CD_REQUIRE((dg == nullptr) == (dbeta == nullptr), "cd_layernorm_bwd: dg and dbeta are both given or both NULL");
+  const size_t smem = dg ? sizeof(float) * 2 * C : 0;
   const int slots = nq <= 32 ? 1 : cd_cdiv(nq, 32);
-#define CD_LNB(N, P) layernorm_bwd_kernel<N, P><<<blocks, 256, smem, st>>>(dy, dy_ld, h, h_ld, stats, g, npix, C, addend, addend_ld, dh, dh_ld, dg, dbeta, ppb)
+#define CD_LNB(N, P) do { \
+    if (dg) layernorm_bwd_kernel<N, P, true><<<blocks, 256, smem, st>>>(dy, dy_ld, h, h_ld, stats, g, npix, C, addend, addend_ld, dh, dh_ld, dg, dbeta, ppb); \
+    else layernorm_bwd_kernel<N, P, false><<<blocks, 256, smem, st>>>(dy, dy_ld, h, h_ld, stats, g, npix, C, addend, addend_ld, dh, dh_ld, dg, dbeta, ppb); \
+  } while (0)
   if (slots == 1) CD_LNB(1, 4); else if (slots == 2) CD_LNB(2, 2); else if (slots <= 4) CD_LNB(4, 1); else CD_LNB(8, 1);
 #undef CD_LNB
   CD_LAUNCH_CHECK();

@@ -861,11 +861,16 @@ __global__ void upsample_nearest2x_kernel(const float* __restrict__ x, int x_ld,
   }
 }
 
-__global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, int ld, int B, int HW, int C, float* __restrict__ out) {
+// out (NCHW) = x (NHWC, row stride ld) [+ add (NCHW, same shape as out)]
+__global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, int ld, int B, int HW, int C, const float* __restrict__ add,
+                                    float* __restrict__ out) {
   const long long pix = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (pix >= static_cast<long long>(B) * HW) return;
   const int b = static_cast<int>(pix / HW), p = static_cast<int>(pix % HW);
-  for (int c = 0; c < C; ++c) out[(static_cast<long long>(b) * C + c) * HW + p] = x[pix * ld + c];
+  for (int c = 0; c < C; ++c) {
+    const long long o = (static_cast<long long>(b) * C + c) * HW + p;
+    out[o] = add ? x[pix * ld + c] + add[o] : x[pix * ld + c];
+  }
 }
 
 // generalised time MLP: emb(dim) -> hid (act) -> tdim ; cond_all = Wc act(temb) + bc.  act: 0 gelu, 1 swish
@@ -1089,11 +1094,14 @@ extern "C" int cd_upsample_nearest2x(const float* x, int x_ld, int B, int H, int
   CD_LAUNCH_CHECK();
   return 0;
 }
-extern "C" int cd_nhwc_to_nchw(const float* x, int ld, int B, int H, int W, int C, float* out, void* stream) {
+extern "C" int cd_nhwc_to_nchw_add(const float* x, int ld, int B, int H, int W, int C, const float* add, float* out, void* stream) {
   const long long npix = static_cast<long long>(B) * H * W;
-  nhwc_to_nchw_kernel<<<cd_cdiv(npix, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(x, ld, B, H * W, C, out);
+  nhwc_to_nchw_kernel<<<cd_cdiv(npix, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(x, ld, B, H * W, C, add, out);
   CD_LAUNCH_CHECK();
   return 0;
+}
+extern "C" int cd_nhwc_to_nchw(const float* x, int ld, int B, int H, int W, int C, float* out, void* stream) {
+  return cd_nhwc_to_nchw_add(x, ld, B, H, W, C, nullptr, out, stream);
 }
 extern "C" int cd_time_mlp2_fwd(const int64_t* t, int B, int dim, int hid, int tdim, int act, const float* w1, const float* b1,
                                 const float* w2, const float* b2, const float* wc, const float* bc, int sumC, float* temb,

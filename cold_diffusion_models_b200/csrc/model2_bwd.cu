@@ -25,6 +25,9 @@ __device__ __forceinline__ float gn_lane_sum(const float (*v)[512], int c, int n
 //   dx = rstd_g * (dz*gamma - mean_g(dz*gamma) - xh * mean_g(dz*gamma*xh));  dcond[b][c] = sum_pixels dx
 // mean_g and rstd_g come from cd_gn_plane_stats, as in the forward (the same bits); every sum within the CTA is added in a fixed
 // order (gn_lane_sum), so the result does not depend on the order the threads run in.
+// kParams = false (dgamma = dbeta = NULL, frozen gamma and beta): the parameter accumulation is compiled out; dx and dcond are
+// the same bits as with it.
+template <bool kParams>
 __global__ void __launch_bounds__(512)
 groupnorm_bwd_kernel(const float* __restrict__ x, int x_ld, int HW, int C, int groups, const float* __restrict__ cond, int cond_ld,
                      const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int swish,
@@ -69,8 +72,10 @@ groupnorm_bwd_kernel(const float* __restrict__ x, int x_ld, int HW, int C, int g
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     cdz[c] = gn_lane_sum(ta, c, nq, np); cdzx[c] = gn_lane_sum(tb, c, nq, np);
-    atomicAdd(dgamma + c, cdzx[c]);
-    atomicAdd(dbeta + c, cdz[c]);
+    if constexpr (kParams) {
+      atomicAdd(dgamma + c, cdzx[c]);
+      atomicAdd(dbeta + c, cdz[c]);
+    }
   }
   __syncthreads();
   for (int g = threadIdx.x; g < groups; g += blockDim.x) {
@@ -232,13 +237,15 @@ gn_split_bwd_dx_kernel(const float* __restrict__ x, int x_ld, long long HW, int 
   for (int c = threadIdx.x; c < C; c += blockDim.x) dpart[(static_cast<long long>(b) * nch + k) * C + c] = gn_lane_sum(tdx, c, nq, np);
 }
 
-// blocks b < B (with dcond): dcond[b][c] = sum over chunks of dpart; the last block: dgamma / dbeta += sum over images of csum
+// blocks b < B (with dcond): dcond[b][c] = sum over chunks of dpart; the last block (kParams): dgamma / dbeta += sum over images
+// of csum
+template <bool kParams>
 __global__ void __launch_bounds__(512)
 gn_split_bwd_final_kernel(const float* __restrict__ csum, int B, int C, const float* __restrict__ dpart, int nch,
                           float* __restrict__ dcond, int dcond_ld, float* __restrict__ dgamma, float* __restrict__ dbeta) {
   __shared__ float scratch[2048];
   const int b = blockIdx.x;
-  if (b == static_cast<int>(gridDim.x) - 1) {
+  if (kParams && b == static_cast<int>(gridDim.x) - 1) {
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
       float a = 0.f, a2 = 0.f;
       for (int i = 0; i < B; ++i) { a += csum[static_cast<long long>(i) * 2 * C + c]; a2 += csum[static_cast<long long>(i) * 2 * C + C + c]; }
@@ -373,6 +380,8 @@ extern "C" int cd_groupnorm_bwd(const float* x, int x_ld, int B, int64_t HW, int
                                 float* dx, int dx_ld, float* dgamma, float* dbeta, float* dcond, int dcond_ld, void* stream) {
   CD_REQUIRE(C % 4 == 0 && C % groups == 0 && C / 4 <= 512 && x_ld % 4 == 0 && dy_ld % 4 == 0 && dx_ld % 4 == 0 &&
              (!cond || cond_ld % 4 == 0), "cd_groupnorm_bwd: unsupported C=%d groups=%d", C, groups);
+  CD_REQUIRE((dgamma == nullptr) == (dbeta == nullptr), "cd_groupnorm_bwd: dgamma and dbeta are both given or both NULL");
+  const bool params = dgamma != nullptr;
   if (HW > CD_GN_SPLIT_MIN_HW) {
     CD_REQUIRE(B <= 65535, "cd_groupnorm_bwd: the split-plane path takes at most 65535 images (B=%d)", B);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -392,20 +401,28 @@ extern "C" int cd_groupnorm_bwd(const float* x, int x_ld, int B, int64_t HW, int
     gn_split_bwd_dx_kernel<<<dim3(nch, B), 512, 0, st>>>(x, x_ld, HW, C, groups, cond, cond_ld, gamma, beta, swish, dy, dy_ld, cp,
                                                          stats, gab, dx, dx_ld, dpart);
     CD_LAUNCH_CHECK();
-    gn_split_bwd_final_kernel<<<dcond ? B + 1 : 1, 512, 0, st>>>(csum, B, C, dpart, nch, dcond, dcond_ld, dgamma, dbeta);
+    const int fin = (dcond ? B : 0) + (params ? 1 : 0);
+    if (fin == 0) return 0;
+    if (params) gn_split_bwd_final_kernel<true><<<fin, 512, 0, st>>>(csum, B, C, dpart, nch, dcond, dcond_ld, dgamma, dbeta);
+    else gn_split_bwd_final_kernel<false><<<fin, 512, 0, st>>>(csum, B, C, dpart, nch, dcond, dcond_ld, dgamma, dbeta);
     CD_LAUNCH_CHECK();
     return 0;
   }
   // dynamic shared memory beyond 48 KB less the kernel's 16 KB of static scratch (4 * groups + 2 * C > 8192, e.g. groups == C
   // above 1365) needs the opt-in; at most 48 KB + 16 KB
   const size_t smem = sizeof(float) * (4 * groups + 2 * C);
-  static size_t attr = 0;
-  if (smem > 32 * 1024 && smem > attr) {
-    CD_CUDA(cudaFuncSetAttribute(groupnorm_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = smem;
+  static size_t attr[2] = {0, 0};
+  if (smem > 32 * 1024 && smem > attr[params]) {
+    CD_CUDA(cudaFuncSetAttribute(params ? groupnorm_bwd_kernel<true> : groupnorm_bwd_kernel<false>,
+                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr[params] = smem;
   }
-  groupnorm_bwd_kernel<<<B, 512, smem, static_cast<cudaStream_t>(stream)>>>(x, x_ld, (int)HW, C, groups, cond, cond_ld, gamma, beta, eps, swish,
-                                                                         dy, dy_ld, dx, dx_ld, dgamma, dbeta, dcond, dcond_ld);
+  if (params)
+    groupnorm_bwd_kernel<true><<<B, 512, smem, static_cast<cudaStream_t>(stream)>>>(x, x_ld, (int)HW, C, groups, cond, cond_ld, gamma, beta,
+                                                                                 eps, swish, dy, dy_ld, dx, dx_ld, dgamma, dbeta, dcond, dcond_ld);
+  else
+    groupnorm_bwd_kernel<false><<<B, 512, smem, static_cast<cudaStream_t>(stream)>>>(x, x_ld, (int)HW, C, groups, cond, cond_ld, gamma, beta,
+                                                                                  eps, swish, dy, dy_ld, dx, dx_ld, dgamma, dbeta, dcond, dcond_ld);
   CD_LAUNCH_CHECK();
   return 0;
 }

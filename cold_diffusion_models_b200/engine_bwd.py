@@ -5,6 +5,9 @@ sm_90a kernels: data-gradients of the dense convolutions are tap-list convolutio
 packed weights (cd_conv_fwd), weight-gradients are cd_conv_wgrad, and the HBM-bound pieces have dedicated
 kernels (backward.cu).  Parameter gradients are ACCUMULATED into reference-layout views of one flat fp32
 buffer (`engine.flat_grad`), which is what the optimizer / the NCCL all-reduce consume.
+
+Only parameters with requires_grad get a gradient: every weight-gradient launch of a frozen parameter is skipped and its slice
+of the buffer is never written.  The gradient with respect to the network input is formed on request (`need_dx`).
 """
 import ctypes as C
 import torch
@@ -103,9 +106,12 @@ class BackwardMixin:
         self.mark_weights_dirty()
 
     def attach_grads(self):
-        """make every parameter's .grad a view of the flat buffer (zeroing slices that were detached)."""
+        """make every trainable parameter's .grad a view of the flat buffer (zeroing slices that were detached); frozen
+        parameters (requires_grad=False) keep theirs (None)."""
         self._setup_grads()
         for n, p in self.unet.named_parameters():
+            if not p.requires_grad:
+                continue
             g = self.G[n]
             if p.grad is None or p.grad.data_ptr() != g.data_ptr():
                 g.zero_()
@@ -168,8 +174,13 @@ class BackwardMixin:
                transposed_conv=False, key=None, real_c=None):
         """accumulate the weight (and bias) gradient of one tap-list convolution into reference-layout grads.
         real_c: `src` is a zero-padded view of an activation with only real_c channels (image-edge block): the tensor-core
-        kernel writes the padded gradient into a scratch buffer whose first real_c columns are then added to the packed gradient."""
+        kernel writes the padded gradient into a scratch buffer whose first real_c columns are then added to the packed gradient.
+        wgrad_param / bias_param None: that parameter is frozen (both None: nothing runs)."""
         nt = len(taps)
+        if wgrad_param is None:
+            if bias_param is not None and out_map == (1, 1, 0, 0):
+                call('cd_colsum', C.c_void_p(dout.addr()), dout.ld, C.c_int64(grid[0] * grid[1] * grid[2]), Cout, ptr(bias_param), stream())
+            return
         if real_c is not None:
             pk = self.Gp[wgrad_param.data_ptr()]
             tmp = self.buf('dwp.pad.' + key, (nt, Cout, src.C))
@@ -212,12 +223,20 @@ class BackwardMixin:
             else:
                 ub.add(dwp, taps, wgrad_param, shape=tuple(wgrad_param.shape), transposed_conv=transposed_conv)
 
+    def _gt(self, name):
+        """gradient view of parameter `name`, or None when it is frozen in the running backward"""
+        return self.G[name] if self._train is None or name in self._train else None
+
+    def _scratch(self, name, n):
+        """write-only stand-in for the gradient of a frozen parameter that a fused kernel produces together with a data gradient"""
+        return self.buf('g.scratch.' + name, (n,))
+
     def _block_bwd(self, bs, save, dyv, need_dx=True):
         sv = save[bs.name]
         xv, hv, uv, prev, stats, hpre = sv['x'], sv['hn'], sv['u'], sv['pre'], sv['stats'], sv['hpre']
         B, H, W = xv.B, xv.H, xv.W
         m = bs.mod
-        P, G = self._packed, self.G
+        P, gt = self._packed, self._gt
         pn = bs.name
         grid = (B, H, W)
         # ---- conv2 (+ res_conv) ----
@@ -225,21 +244,25 @@ class BackwardMixin:
         edge_c = bs.din if xpad is not None else None
         if bs.has_res:
             # conv2 and res_conv add into the same output: one column sum of dy feeds both bias gradients
-            tmp = self.buf('g.dbias', (max(b_.dout for b_ in self.blocks.values()),))
-            tmp.zero_()
-            self._wgrad(uv, T3, bs.dout, grid, dyv, G[pn + '.net.3.weight'], tmp, key=pn + '.w2')
-            self._wgrad(xpad if xpad is not None else xv, T1, bs.dout, grid, dyv, G[pn + '.res_conv.weight'], None, key=pn + '.wr',
+            gb = [(leaf, gt(pn + leaf)) for leaf in ('.net.3.bias', '.res_conv.bias')]
+            gb = [(leaf, g) for leaf, g in gb if g is not None]
+            tmp = None
+            if gb:
+                tmp = self.buf('g.dbias', (max(b_.dout for b_ in self.blocks.values()),))
+                tmp.zero_()
+            self._wgrad(uv, T3, bs.dout, grid, dyv, gt(pn + '.net.3.weight'), tmp, key=pn + '.w2')
+            self._wgrad(xpad if xpad is not None else xv, T1, bs.dout, grid, dyv, gt(pn + '.res_conv.weight'), None, key=pn + '.wr',
                         real_c=edge_c)
-            for leaf in ('.net.3.bias', '.res_conv.bias'):
-                call('cd_add', ptr(G[pn + leaf]), bs.dout, ptr(tmp), bs.dout, ptr(G[pn + leaf]), bs.dout, C.c_int64(1), bs.dout, stream())
+            for leaf, g in gb:
+                call('cd_add', ptr(g), bs.dout, ptr(tmp), bs.dout, ptr(g), bs.dout, C.c_int64(1), bs.dout, stream())
         else:
-            self._wgrad(uv, T3, bs.dout, grid, dyv, G[pn + '.net.3.weight'], G[pn + '.net.3.bias'], key=pn + '.w2')
+            self._wgrad(uv, T3, bs.dout, grid, dyv, gt(pn + '.net.3.weight'), gt(pn + '.net.3.bias'), key=pn + '.w2')
         dpre = self.buf('g.pre.%dx%dx%d' % (H, W, bs.dmid), (B, H, W, bs.dmid))
         d = ops.make_conv_desc([(dyv, T3D, P[pn + '.w2T'], False)], View(dpre), grid, Cout=bs.dmid,
                                act=ACT_GELU_BWD, aux=prev)
         self._conv(d, _tc_ok(bs.dout))
         # ---- conv1 ----
-        self._wgrad(hv, T3, bs.dmid, grid, View(dpre), G[pn + '.net.1.weight'], G[pn + '.net.1.bias'], key=pn + '.w1', real_c=edge_c)
+        self._wgrad(hv, T3, bs.dmid, grid, View(dpre), gt(pn + '.net.1.weight'), gt(pn + '.net.1.bias'), key=pn + '.w1', real_c=edge_c)
         ld_in = sv.get('ld_h', hv.ld)
         dhn = self.buf('g.hn.%dx%dx%d' % (H, W, ld_in), (B, H, W, ld_in))
         d = ops.make_conv_desc([(View(dpre), T3D, P[pn + '.w1T'], False)], View(dhn, 0, bs.din), grid, Cout=bs.din)
@@ -247,20 +270,25 @@ class BackwardMixin:
         # ---- LayerNorm ----
         if bs.has_norm:
             dh = self.buf('g.h.%dx%dx%d' % (H, W, ld_in), (B, H, W, ld_in))
+            dg, db = self._ln_grads(pn + '.net.0', bs.din)
             call('cd_layernorm_bwd', ptr(dhn), ld_in, ptr(hpre), ld_in, ptr(stats), ptr(m.net[0].g), C.c_int64(B * H * W),
-                 bs.din, NULL, 0, ptr(dh), ld_in, ptr(G[pn + '.net.0.g']), ptr(G[pn + '.net.0.b']), stream())
+                 bs.din, NULL, 0, ptr(dh), ld_in, ptr(dg), ptr(db), stream())
         else:
             dh = dhn
         # ---- time conditioning + depthwise bias ----
+        dsb = gt(pn + '.ds_conv.bias')
         if bs.cond_off is not None:
-            dslice = C.c_void_p(self._dcond.data_ptr() + 4 * bs.cond_off)
-            call('cd_colsum_batched', ptr(dh), ld_in, B, C.c_int64(H * W), bs.din, dslice, self.sumC, stream())
-            # d(ds_conv.bias) = sum_b dcond[b]  (same per-pixel gradient, already reduced over pixels)
-            call('cd_colsum', dslice, self.sumC, C.c_int64(B), bs.din, ptr(G[pn + '.ds_conv.bias']), stream())
-        else:
-            call('cd_colsum', ptr(dh), ld_in, C.c_int64(B * H * W), bs.din, ptr(G[pn + '.ds_conv.bias']), stream())
-        call('cd_dwconv7_wgrad', ptr(dh), ld_in, C.c_void_p(xv.addr()), xv.ld, B, H, W, bs.din,
-             ptr(G[pn + '.ds_conv.weight']), stream())
+            if self._time_train or dsb is not None:
+                dslice = C.c_void_p(self._dcond.data_ptr() + 4 * bs.cond_off)
+                call('cd_colsum_batched', ptr(dh), ld_in, B, C.c_int64(H * W), bs.din, dslice, self.sumC, stream())
+                # d(ds_conv.bias) = sum_b dcond[b]  (same per-pixel gradient, already reduced over pixels)
+                if dsb is not None:
+                    call('cd_colsum', dslice, self.sumC, C.c_int64(B), bs.din, ptr(dsb), stream())
+        elif dsb is not None:
+            call('cd_colsum', ptr(dh), ld_in, C.c_int64(B * H * W), bs.din, ptr(dsb), stream())
+        dsw = gt(pn + '.ds_conv.weight')
+        if dsw is not None:
+            call('cd_dwconv7_wgrad', ptr(dh), ld_in, C.c_void_p(xv.addr()), xv.ld, B, H, W, bs.din, ptr(dsw), stream())
         if not need_dx:
             return None
         # ---- dx = dwconv7^T(dh) + residual path ----
@@ -276,9 +304,18 @@ class BackwardMixin:
             call('cd_dwconv7_fwd', ptr(dh), ld_in, B, H, W, bs.din, ptr(m.ds_conv.weight), NULL, NULL, 0, ptr(dx), ld_in, 1,
                  C.c_void_p(addv.addr()), addv.ld, stream())
         else:
+            # image-edge block (din = 1 or 3 image channels, rows of ld_in = 4 floats): the flipped 7x7 on CUDA cores
             call('cd_dwconv7_ln_fwd', ptr(dh), ld_in, B, H, W, bs.din, ptr(m.ds_conv.weight), NULL, NULL, 0, NULL, NULL,
                  C.c_float(0.0), ptr(dx), ld_in, NULL, NULL, 0, 0, 1, C.c_void_p(addv.addr()), addv.ld, stream())
         return View(dx, 0, bs.din)
+
+    def _ln_grads(self, prefix, n):
+        """(dg, db) pointers of a LayerNorm backward: the gradient views, NULL for both when both are frozen (the kernel then
+        skips the parameter reduction), a scratch stand-in for the frozen one of a half-frozen pair"""
+        dg, db = self._gt(prefix + '.g'), self._gt(prefix + '.b')
+        if dg is None and db is None:
+            return None, None
+        return (dg if dg is not None else self._scratch('ln.g', n)), (db if db is not None else self._scratch('ln.b', n))
 
     def _attn_bwd(self, spec, save, dyv):
         sv = save[spec.name]
@@ -287,11 +324,14 @@ class BackwardMixin:
         n = H * W
         dim = spec.dim
         a = spec.attn
-        P, G = self._packed, self.G
+        P = self._packed
         pn = spec.name + '.fn'
         grid = (B, H, W)
         tc_pb = n >= 128
-        call('cd_colsum', C.c_void_p(dyv.addr()), dyv.ld, C.c_int64(B * n), dim, ptr(G[pn + '.fn.to_out.bias']), stream())
+        gt = self._gt
+        ob = gt(pn + '.fn.to_out.bias')
+        if ob is not None:
+            call('cd_colsum', C.c_void_p(dyv.addr()), dyv.ld, C.c_int64(B * n), dim, ptr(ob), stream())
         # dweff[b][co][hd] = sum_pix dy[pix][co] * q[pix][hd]
         dweff = self.buf('g.dweff', (B, dim, 128))
         dweff.zero_()
@@ -307,8 +347,9 @@ class BackwardMixin:
             ops.conv_wgrad(d, dyv, dweff, None, impl=self.conv_impl)
         dctxn = self.buf('g.dctxn', (B, 4, 32, 32))
         rowdot = self.buf('g.rowdot', (B, 128))
+        ow = gt(pn + '.fn.to_out.weight')
         call('cd_linattn_bwd_small', ptr(dweff), ptr(ctx), ptr(ksum), ptr(a.to_out.weight), B, dim, C.c_float(a.scale),
-             ptr(G[pn + '.fn.to_out.weight']), ptr(dctxn), ptr(rowdot), stream())
+             ptr(ow if ow is not None else self._scratch('to_out.%d' % dim, dim * 128)), ptr(dctxn), ptr(rowdot), stream())
         dqkv = self.buf('g.qkv.%dx%d' % (H, W), (B, H, W, 384))
         wt = self.buf('g.wefft', (B, 128, dim))
         call('cd_transpose_weff', ptr(weff), B, dim, ptr(wt), stream())
@@ -316,19 +357,30 @@ class BackwardMixin:
         self._conv(d, tc_pb and _tc_ok(dim))
         call('cd_linattn_bwd_kv', ptr(qkv), 384, B, n, ptr(kmax), ptr(ksum), ptr(dctxn), ptr(rowdot), ptr(dqkv), 384, stream())
         # to_qkv
-        self._wgrad(xnv, T1, 384, grid, View(dqkv), G[pn + '.fn.to_qkv.weight'], None, key=spec.name + '.wqkv')
+        self._wgrad(xnv, T1, 384, grid, View(dqkv), gt(pn + '.fn.to_qkv.weight'), None, key=spec.name + '.wqkv')
         dxn = self.buf('g.xn.%dx%dx%d' % (H, W, dim), (B, H, W, dim))
         d = ops.make_conv_desc([(View(dqkv), T1, P[spec.name + '.wqkvT'], False)], View(dxn), grid, Cout=dim)
         self._conv(d, True)
         dx = self.buf('g.x.' + spec.name, (B, H, W, dim))
+        dg, db = self._ln_grads(pn + '.norm', dim)
         call('cd_layernorm_bwd', ptr(dxn), dim, C.c_void_p(xv.addr()), xv.ld, ptr(stats), ptr(spec.norm.g), C.c_int64(B * n),
-             dim, C.c_void_p(dyv.addr()), dyv.ld, ptr(dx), dim, ptr(G[pn + '.norm.g']), ptr(G[pn + '.norm.b']), stream())
+             dim, C.c_void_p(dyv.addr()), dyv.ld, ptr(dx), dim, ptr(dg), ptr(db), stream())
         return View(dx)
 
     # ------------------------------------------------------------------------------------------
-    def backward(self, save, dout):
-        """dout: (B, out_dim, H, W) NCHW gradient of the network output.  Accumulates into self.G."""
+    _train = None              # names of the trainable parameters in the running backward (None: all)
+    _time_train = True         # some parameter of the time path (time_mlp.*, *.mlp.1.*) is trainable
+
+    def backward(self, save, dout, need_dx=False, trainable=None):
+        """dout: (B, out_dim, H, W) NCHW gradient of the network output.  Accumulates the gradients of the parameters named in
+        `trainable` (None: every parameter) into self.G.  need_dx: also returns the gradient of the input x (B, C, H, W) NCHW,
+        else None."""
         unet = self.unet
+        names = [n for n, _ in unet.named_parameters()]
+        if trainable is not None and len(set(trainable)) == len(names):
+            trainable = None
+        self._train = None if trainable is None else set(trainable)
+        self._time_train = any(self._gt(n) is not None for n in names if n.startswith('time_mlp.') or '.mlp.1.' in n)
         shape, gen = save.get('_gen', (None, None))
         if shape is not None and self._gen_by_shape.get(shape) != gen:
             raise RuntimeError("Unet backward: another forward with input shape %r ran on this network after the forward being "
@@ -336,7 +388,7 @@ class BackwardMixin:
                                "backward() before the next forward (e.g. accumulate micro-batches one at a time)" % (shape,))
         self._setup_grads()
         self.prepare_weights_bwd()
-        P, G = self._packed, self.G
+        P = self._packed
         dout = dout.contiguous().float()
         B = dout.shape[0]
         # packed weight gradients: unpacked one by one right after each wgrad, or (COLDDIFF_BATCHED_REPACK) all at once below
@@ -353,8 +405,10 @@ class BackwardMixin:
         h, w = fx.H, fx.W
         dfo = self.buf('g.final', (B, h, w, fx.ld))
         od = self.final_proj.weight.shape[0]
+        fw, fb = self._gt('final_conv.1.weight'), self._gt('final_conv.1.bias')
         call('cd_conv1x1_to_nchw_bwd', ptr(dout), ptr(fx.t), fx.ld, B, h, w, fx.C, ptr(self.final_proj.weight), od,
-             ptr(dfo), fx.ld, ptr(G['final_conv.1.weight']), ptr(G['final_conv.1.bias']), stream())
+             ptr(dfo), fx.ld, ptr(fw if fw is not None else self._scratch('final.w', od * fx.C)),
+             ptr(fb if fb is not None else self._scratch('final.b', od)), stream())
         d = self._block_bwd(self.final_block, save, View(dfo))
         # ---- up path ----
         dskip = {}
@@ -366,9 +420,11 @@ class BackwardMixin:
                 c = xv.C
                 hh, ww = xv.H, xv.W
                 # bias
-                call('cd_colsum', C.c_void_p(d.addr()), d.ld, C.c_int64(B * d.H * d.W), c, ptr(G['ups.%d.3.bias' % k]), stream())
+                ub = self._gt('ups.%d.3.bias' % k)
+                if ub is not None:
+                    call('cd_colsum', C.c_void_p(d.addr()), d.ld, C.c_int64(B * d.H * d.W), c, ptr(ub), stream())
                 for (py, px), tp in TPAR.items():
-                    self._wgrad(xv, tp, c, (B, hh, ww), d, G['ups.%d.3.weight' % k], None, out_map=(2, 2, py, px),
+                    self._wgrad(xv, tp, c, (B, hh, ww), d, self._gt('ups.%d.3.weight' % k), None, out_map=(2, 2, py, px),
                                 transposed_conv=True, key='ups.%d.3.%d%d' % (k, py, px))
                 dxu = self.buf('g.up%d' % k, (B, hh, ww, c))
                 dd = ops.make_conv_desc([(d, T4, P['ups.%d.3T' % k], False)], View(dxu), (B, hh, ww), stride=2, Cout=c)
@@ -394,7 +450,7 @@ class BackwardMixin:
                 xv = sv['x']
                 c = xv.C
                 hh, ww = xv.H, xv.W
-                self._wgrad(xv, T4, c, (B, hh // 2, ww // 2), d, G['downs.%d.3.weight' % i], G['downs.%d.3.bias' % i],
+                self._wgrad(xv, T4, c, (B, hh // 2, ww // 2), d, self._gt('downs.%d.3.weight' % i), self._gt('downs.%d.3.bias' % i),
                             stride=2, key='downs.%d.3' % i)
                 dsv = self.buf('g.dn%d' % i, (B, hh, ww, c))
                 for (py, px), tp in TPAR.items():
@@ -409,15 +465,23 @@ class BackwardMixin:
                 d = View(dsum)
             d = self._attn_bwd(at, save, d)
             d = self._block_bwd(b1, save, d)
-            d = self._block_bwd(b0, save, d, need_dx=(i > 0))
+            d = self._block_bwd(b0, save, d, need_dx=(i > 0 or need_dx))
             if i >= 2:
                 self._grads_ready_from('downs.%d' % i)     # the two coarsest levels carry 22 of the 24 M down-path parameters
         # ---- time MLP ----
-        if unet.time_mlp is not None:
+        if unet.time_mlp is not None and self._time_train:
             self._time_bwd(save)
         if self._unpack_batch is not None:
             self._unpack_batch.run(accumulate=True, clear_src=True)
             self._dwp_pending = False
+        if not need_dx:
+            return None
+        # ---- input gradient: NHWC rows (ld 4 for 1 or 3 image channels) -> NCHW, plus dout for the `x +` of residual=True ----
+        x_in = save['final']['x_in']
+        dx = torch.empty(x_in.shape, device=dout.device, dtype=torch.float32)
+        call('cd_nhwc_to_nchw_add', C.c_void_p(d.addr()), d.ld, B, d.H, d.W, d.C, ptr(dout) if unet.residual else NULL, ptr(dx),
+             stream())
+        return dx
 
     def _grads_ready_from(self, group):
         """tell the trainer that flat_grad[start of `group` : previous mark) holds final values (multi-GPU: the all-reduce of
@@ -435,31 +499,43 @@ class BackwardMixin:
     def _time_bwd(self, save):
         sv = save['time']
         unet = self.unet
-        G, P = self.G, self._packed
+        P = self._packed
         dim = self.dim
         B = sv['temb'].shape[0]
         dcond = self._dcond
         temb, hid_pre, sinemb = sv['temb'], sv['hid'], sv['sinemb']
+        tg = self._gt
         gt = self.buf('g.gt', (B, dim))
-        call('cd_gelu_bwd', NULL, ptr(temb), C.c_int64(B * dim), NULL, ptr(gt), stream())
+        if any(tg(bs.name + '.mlp.1.weight') is not None for bs in self.cond_blocks):
+            call('cd_gelu_bwd', NULL, ptr(temb), C.c_int64(B * dim), NULL, ptr(gt), stream())
         for bs in self.cond_blocks:
-            wname = bs.name + '.mlp.1.weight'
+            gw, gb = tg(bs.name + '.mlp.1.weight'), tg(bs.name + '.mlp.1.bias')
             # dW[c][k] += sum_b dcond[b][off+c] * gt[b][k]
-            call('cd_small_gemm', C.c_void_p(dcond.data_ptr() + 4 * bs.cond_off), self.sumC, 1, ptr(gt), dim, 0,
-                 ptr(G[wname]), dim, bs.din, dim, B, 1, stream())
-            call('cd_colsum', C.c_void_p(dcond.data_ptr() + 4 * bs.cond_off), self.sumC, C.c_int64(B), bs.din,
-                 ptr(G[bs.name + '.mlp.1.bias']), stream())
+            if gw is not None:
+                call('cd_small_gemm', C.c_void_p(dcond.data_ptr() + 4 * bs.cond_off), self.sumC, 1, ptr(gt), dim, 0,
+                     ptr(gw), dim, bs.din, dim, B, 1, stream())
+            if gb is not None:
+                call('cd_colsum', C.c_void_p(dcond.data_ptr() + 4 * bs.cond_off), self.sumC, C.c_int64(B), bs.din, ptr(gb), stream())
+        g1w, g1b, g3w, g3b = (tg('time_mlp.%s' % n) for n in ('1.weight', '1.bias', '3.weight', '3.bias'))
+        if g1w is None and g1b is None and g3w is None and g3b is None:
+            return
         dgt = self.buf('g.dgt', (B, dim))
         call('cd_small_gemm', ptr(dcond), self.sumC, 0, ptr(P['cond.w']), dim, 0, ptr(dgt), dim, B, dim, self.sumC, 0, stream())
         dtemb = self.buf('g.dtemb', (B, dim))
         call('cd_gelu_bwd', ptr(dgt), ptr(temb), C.c_int64(B * dim), ptr(dtemb), NULL, stream())
         l1, l2 = unet.time_mlp[1], unet.time_mlp[3]
-        hact = self.buf('g.hact', (B, 4 * dim))
-        call('cd_gelu_bwd', NULL, ptr(hid_pre), C.c_int64(B * 4 * dim), NULL, ptr(hact), stream())
-        call('cd_small_gemm', ptr(dtemb), dim, 1, ptr(hact), 4 * dim, 0, ptr(G['time_mlp.3.weight']), 4 * dim, dim, 4 * dim, B, 1, stream())
-        call('cd_colsum', ptr(dtemb), dim, C.c_int64(B), dim, ptr(G['time_mlp.3.bias']), stream())
+        if g3w is not None:
+            hact = self.buf('g.hact', (B, 4 * dim))
+            call('cd_gelu_bwd', NULL, ptr(hid_pre), C.c_int64(B * 4 * dim), NULL, ptr(hact), stream())
+            call('cd_small_gemm', ptr(dtemb), dim, 1, ptr(hact), 4 * dim, 0, ptr(g3w), 4 * dim, dim, 4 * dim, B, 1, stream())
+        if g3b is not None:
+            call('cd_colsum', ptr(dtemb), dim, C.c_int64(B), dim, ptr(g3b), stream())
+        if g1w is None and g1b is None:
+            return
         dh = self.buf('g.dhid', (B, 4 * dim))
         call('cd_small_gemm', ptr(dtemb), dim, 0, ptr(l2.weight), 4 * dim, 0, ptr(dh), 4 * dim, B, 4 * dim, dim, 0, stream())
         call('cd_gelu_bwd', ptr(dh), ptr(hid_pre), C.c_int64(B * 4 * dim), ptr(dh), NULL, stream())
-        call('cd_small_gemm', ptr(dh), 4 * dim, 1, ptr(sinemb), dim, 0, ptr(G['time_mlp.1.weight']), dim, 4 * dim, dim, B, 1, stream())
-        call('cd_colsum', ptr(dh), 4 * dim, C.c_int64(B), 4 * dim, ptr(G['time_mlp.1.bias']), stream())
+        if g1w is not None:
+            call('cd_small_gemm', ptr(dh), 4 * dim, 1, ptr(sinemb), dim, 0, ptr(g1w), dim, 4 * dim, dim, B, 1, stream())
+        if g1b is not None:
+            call('cd_colsum', ptr(dh), 4 * dim, C.c_int64(B), 4 * dim, ptr(g1b), stream())

@@ -307,7 +307,7 @@ class Model(nn.Module):
             if getattr(self, 'with_time_emb', True):
                 raise ValueError("Model.forward needs t unless the model was built with with_time_emb=False")
             t = torch.zeros(x.shape[0], dtype=torch.int64, device=x.device)
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
             from . import model2_train
             return model2_train.ModelFunction.apply(self, x, t, *self.engine.param_list())
         assert x.shape[2] == x.shape[3] == self.resolution

@@ -9,6 +9,9 @@ consistency and one Trainer step.
 Gradient routing: every activation that the forward writes into a (slice of a) buffer has a gradient buffer of the same shape;
 consumers ADD into it (dense data-gradient convolutions accumulate through their `resid` input, the rest through cd_add) and the
 producer reads it once all consumers ran -- the reverse of the forward order guarantees that.
+
+Only parameters with requires_grad get a gradient (the weight-gradient launches of frozen ones are skipped); the gradient of the
+input x is formed on request, through the data gradient of conv_in.
 """
 import ctypes as C
 import os
@@ -18,6 +21,7 @@ from . import ops
 from .ops import View, CONV_TC, CONV_SIMT
 from ._lib import call, ptr, stream
 from .engine_bwd import flat_offsets
+from .autograd import check_first_order, trainable_names, once_differentiable
 from .model2 import T1, T3, TDOWN
 
 NULL = C.c_void_p(0)
@@ -72,8 +76,11 @@ class ModelEngine:
         self.mark_weights_dirty()
 
     def attach_grads(self):
+        """.grad of every trainable parameter = its view of the flat buffer; frozen parameters keep theirs (None)"""
         self._setup_grads()
         for n, p in self.model.named_parameters():
+            if not p.requires_grad:
+                continue
             g = self.G[n]
             if p.grad is None or p.grad.data_ptr() != g.data_ptr():
                 g.zero_()
@@ -97,12 +104,16 @@ class ModelFunction(torch.autograd.Function):
         return out
 
     @staticmethod
+    @once_differentiable
     def backward(ctx, dout):
+        check_first_order(dout, "Model backward")
         eng = ctx.model.engine
         eng.attach_grads()
-        backward(ctx.model, ctx.save, dout)
+        need_dx = ctx.needs_input_grad[1]
+        dx = backward(ctx.model, ctx.save, dout, need_dx=need_dx,
+                      trainable=trainable_names(ctx.model.named_parameters(), ctx.needs_input_grad))
         ctx.save = None
-        return (None, None, None) + (None,) * ctx.nparams
+        return (None, dx if need_dx else None, None) + (None,) * ctx.nparams
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -158,7 +169,12 @@ def _colsum(v, out):
 
 
 def _wgrad(m, key, src, taps, Cout, grid, dout, wgrad_param, bias_param, *, stride=1):
-    """accumulate the weight (and bias) gradient of one tap-list convolution into reference-layout (OIHW) gradients"""
+    """accumulate the weight (and bias) gradient of one tap-list convolution into reference-layout (OIHW) gradients; a None
+    gradient is a frozen parameter"""
+    if wgrad_param is None:
+        if bias_param is not None:
+            _colsum(dout, bias_param)
+        return
     nt = len(taps)
     if nt == 1:
         dwp = wgrad_param                                   # 1x1: packed layout == OIHW layout
@@ -182,9 +198,13 @@ def _gn_bwd(m, xv, norm, swish, dyv, dxv, G, gname, cond=None, dcond=None):
     B, H, W = xv.B, xv.H, xv.W
     condp = C.c_void_p(cond) if cond is not None else NULL
     dcondp = C.c_void_p(dcond) if dcond is not None else NULL
+    dg, db = G.get(gname + '.weight'), G.get(gname + '.bias')
+    if (dg is None) != (db is None):            # half-frozen pair: a scratch stand-in for the frozen one
+        scratch = m._buf('g.scratch.gn', (xv.C,))
+        dg, db = (scratch if dg is None else dg), (scratch if db is None else db)
     call('cd_groupnorm_bwd', C.c_void_p(xv.addr()), xv.ld, B, C.c_int64(H * W), xv.C, norm.num_groups, condp, m._sumC,
          ptr(norm.weight), ptr(norm.bias), C.c_float(norm.eps), int(swish), C.c_void_p(dyv.addr()), dyv.ld,
-         C.c_void_p(dxv.addr()), dxv.ld, ptr(G[gname + '.weight']), ptr(G[gname + '.bias']), dcondp, m._sumC, stream())
+         C.c_void_p(dxv.addr()), dxv.ld, ptr(dg), ptr(db), dcondp, m._sumC, stream())
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -216,20 +236,21 @@ def _res_fwd(m, name, b, xv, outv, cond_all, save):
     save[name] = dict(x=xv, n1=n1, h1=h1, n2=n2, seed=seed, p=p)
 
 
-def _res_bwd(m, name, b, save, dyv, dx_acc, dcond_all, cond_all):
-    """dyv: gradient of the block output (read only); dx_acc: gradient buffer of the block input (accumulated into)"""
+def _res_bwd(m, name, b, save, dyv, dx_acc, dcond_all, cond_all, G):
+    """dyv: gradient of the block output (read only); dx_acc: gradient buffer of the block input (accumulated into);
+    G: gradient views of the trainable parameters"""
     sv = save[name]
     xv, n1, h1, n2 = sv['x'], sv['n1'], sv['h1'], sv['n2']
     B, H, W = xv.B, xv.H, xv.W
     grid = (B, H, W)
-    P, G = m._packed, m.engine.G
+    P = m._packed
     cin, cout = b.in_channels, b.out_channels
     # ---- conv2 (+ shortcut): weights, biases
     sc = 'nin_shortcut' if hasattr(b, 'nin_shortcut') else ('conv_shortcut' if hasattr(b, 'conv_shortcut') else None)
-    _wgrad(m, name + '.c2', n2, T3, cout, grid, dyv, G[name + '.conv2.weight'], G[name + '.conv2.bias'])
+    _wgrad(m, name + '.c2', n2, T3, cout, grid, dyv, G.get(name + '.conv2.weight'), G.get(name + '.conv2.bias'))
     if cin != cout:
         taps_sc = T1 if sc == 'nin_shortcut' else T3
-        _wgrad(m, name + '.sc', xv, taps_sc, cout, grid, dyv, G[name + '.%s.weight' % sc], G[name + '.%s.bias' % sc])
+        _wgrad(m, name + '.sc', xv, taps_sc, cout, grid, dyv, G.get(name + '.%s.weight' % sc), G.get(name + '.%s.bias' % sc))
     # ---- through conv2 -> dropout -> swish(GroupNorm2(h1 + cond))
     dn2 = View(m._buf('g.n2.%dx%dx%d' % (H, W, cout), (B, H, W, cout)))
     _dgrad_into(m, dyv, T3D, P[name + '.c2T'], dn2, grid, cout, False)
@@ -238,9 +259,9 @@ def _res_bwd(m, name, b, save, dyv, dx_acc, dcond_all, cond_all):
              C.c_void_p(dn2.addr()), dn2.ld, stream())
     dh1 = View(m._buf('g.h1.%dx%dx%d' % (H, W, cout), (B, H, W, cout)))
     _gn_bwd(m, h1, b.norm2, True, dn2, dh1, G, name + '.norm2', cond=cond_all.data_ptr() + 4 * b._cond_off,
-            dcond=dcond_all.data_ptr() + 4 * b._cond_off)
+            dcond=dcond_all.data_ptr() + 4 * b._cond_off if dcond_all is not None else None)
     # ---- conv1
-    _wgrad(m, name + '.c1', n1, T3, cout, grid, dh1, G[name + '.conv1.weight'], G[name + '.conv1.bias'])
+    _wgrad(m, name + '.c1', n1, T3, cout, grid, dh1, G.get(name + '.conv1.weight'), G.get(name + '.conv1.bias'))
     dn1 = View(m._buf('g.n1.%dx%dx%d' % (H, W, cin), (B, H, W, cin)))
     _dgrad_into(m, dh1, T3D, P[name + '.c1T'], dn1, grid, cin, False)
     dxg = View(m._buf('g.xg.%dx%dx%d' % (H, W, cin), (B, H, W, cin)))
@@ -274,16 +295,16 @@ def _attn_fwd(m, name, a, xv, outv, save):
     save[name] = dict(x=xv, hn=hn, q=q, k=k, v=v, s=s, ho=ho)
 
 
-def _attn_bwd(m, name, a, save, dyv, dx_acc):
+def _attn_bwd(m, name, a, save, dyv, dx_acc, G):
     sv = save[name]
     xv, hn, q, k, v, s, ho = sv['x'], sv['hn'], sv['q'], sv['k'], sv['v'], sv['s'], sv['ho']
     B, H, W = xv.B, xv.H, xv.W
     n, c = H * W, a.in_channels
     grid = (B, H, W)
-    P, G = m._packed, m.engine.G
+    P = m._packed
     scale = int(c) ** (-0.5)
     # proj_out
-    _wgrad(m, name + '.po', ho, T1, c, grid, dyv, G[name + '.proj_out.weight'], G[name + '.proj_out.bias'])
+    _wgrad(m, name + '.po', ho, T1, c, grid, dyv, G.get(name + '.proj_out.weight'), G.get(name + '.proj_out.bias'))
     dho = View(m._buf('g.ah.%dx%d' % (n, c), (B, H, W, c)))
     _dgrad_into(m, dyv, T1, P[name + '.proj_outT'], dho, grid, c, False)
     # h_ = w_ v  (w_ = softmax weights s[b,i,j], M2:176-181)
@@ -308,7 +329,7 @@ def _attn_bwd(m, name, a, save, dyv, dx_acc):
     dhn = View(m._buf('g.an.%dx%d' % (n, c), (B, H, W, c)))
     first = True
     for leaf, g in (('q', dq), ('k', dkv), ('v', dvv)):
-        _wgrad(m, name + '.' + leaf, hn, T1, c, grid, g, G[name + '.%s.weight' % leaf], G[name + '.%s.bias' % leaf])
+        _wgrad(m, name + '.' + leaf, hn, T1, c, grid, g, G.get(name + '.%s.weight' % leaf), G.get(name + '.%s.bias' % leaf))
         _dgrad_into(m, g, T1, P[name + '.' + leaf + 'T'], dhn, grid, c, not first)
         first = False
     dxg = View(m._buf('g.axg.%dx%d' % (n, c), (B, H, W, c)))
@@ -426,10 +447,17 @@ def forward_train(m, x, t, save):
 # ---------------------------------------------------------------------------------------------------------------------
 # backward
 # ---------------------------------------------------------------------------------------------------------------------
-def backward(m, save, dout):
+def backward(m, save, dout, need_dx=False, trainable=None):
+    """dout: NCHW gradient of the output.  Accumulates the gradients of the parameters named in `trainable` (None: all) into the
+    flat buffer; need_dx: returns the NCHW gradient of the input x, else None."""
     top = save['__']
     B, H = top['B'], top['H']
-    P, G = m._packed, m.engine.G
+    P = m._packed
+    G = m.engine.G
+    if trainable is not None:
+        trainable = set(trainable)
+        G = {n: g for n, g in G.items() if n in trainable}
+    time_train = any(n.startswith('temb.') or '.temb_proj.' in n for n in G)
     dout = dout.contiguous().float()
     oc = m.out_ch
     old = oc if oc % 4 == 0 else (oc + 3) // 4 * 4
@@ -450,28 +478,30 @@ def backward(m, save, dout):
     # ---- conv_out and norm_out
     last, no = top['last'], top['no']
     res = last.H
-    _wgrad(m, 'conv_out', no, T3, oc, (B, res, res), dyv, G['conv_out.weight'], G['conv_out.bias'])
+    _wgrad(m, 'conv_out', no, T3, oc, (B, res, res), dyv, G.get('conv_out.weight'), G.get('conv_out.bias'))
     dno = View(m._buf('g.no', (B, res, res, no.C)))
     ops.conv_fwd(ops.make_conv_desc([(dyv, T3D, P['conv_out.T'], False)], dno, (B, res, res), Cout=no.C), CONV_SIMT)
     _gn_bwd(m, last, m.norm_out, True, dno, gview(last), G, 'norm_out')          # first and only writer of d(last)
 
-    dcond_all = m._buf('g.cond', (B, m._sumC)); dcond_all.zero_()
+    dcond_all = None
+    if time_train:                                           # conditioning gradient: only the time path consumes it
+        dcond_all = m._buf('g.cond', (B, m._sumC)); dcond_all.zero_()
     cond_all = top['cond_all']
     for op in reversed(top['ops']):
         kind = op[0]
         if kind == 'res':
             _, name, b, xin, xout = op
-            _res_bwd(m, name, b, save, gview(xout), gview(xin), dcond_all, cond_all)
+            _res_bwd(m, name, b, save, gview(xout), gview(xin), dcond_all, cond_all, G)
         elif kind == 'attn':
             _, name, a, xin, xout = op
-            _attn_bwd(m, name, a, save, gview(xout), gview(xin))
+            _attn_bwd(m, name, a, save, gview(xout), gview(xin), G)
         elif kind == 'up':
             _, i_level, hin, upb, tgt = op
             u = m.up[i_level]
             c, r2 = hin.C, upb.H
             dy = gview(tgt)
-            _wgrad(m, 'up.%d.us' % i_level, upb, T3, c, (B, r2, r2), dy, G['up.%d.upsample.conv.weight' % i_level],
-                   G['up.%d.upsample.conv.bias' % i_level])
+            _wgrad(m, 'up.%d.us' % i_level, upb, T3, c, (B, r2, r2), dy, G.get('up.%d.upsample.conv.weight' % i_level),
+                   G.get('up.%d.upsample.conv.bias' % i_level))
             dup = View(m._buf('g.ups.%d' % i_level, (B, r2, r2, c)))
             _dgrad_into(m, dy, T3D, P['up.%d.usT' % i_level], dup, (B, r2, r2), c, False)
             dsm = View(m._buf('g.upsm.%d' % i_level, (B, r2 // 2, r2 // 2, c)))
@@ -481,8 +511,8 @@ def backward(m, save, dout):
             _, i_level, hin, tgt = op
             c, r = hin.C, hin.H
             dy = gview(tgt)
-            _wgrad(m, 'down.%d.ds' % i_level, hin, TDOWN, c, (B, r // 2, r // 2), dy, G['down.%d.downsample.conv.weight' % i_level],
-                   G['down.%d.downsample.conv.bias' % i_level], stride=2)
+            _wgrad(m, 'down.%d.ds' % i_level, hin, TDOWN, c, (B, r // 2, r // 2), dy, G.get('down.%d.downsample.conv.weight' % i_level),
+                   G.get('down.%d.downsample.conv.bias' % i_level), stride=2)
             dx = gview(hin)
             for py in (0, 1):
                 for px in (0, 1):
@@ -491,27 +521,58 @@ def backward(m, save, dout):
                     ops.conv_fwd(d, m.conv_impl if c % 32 == 0 else CONV_SIMT)
         elif kind == 'conv_in':
             _, xin, hv = op
-            _wgrad(m, 'conv_in', xin, T3, m.ch, (B, H, H), gview(hv), G['conv_in.weight'], G['conv_in.bias'])
+            _wgrad(m, 'conv_in', xin, T3, m.ch, (B, H, H), gview(hv), G.get('conv_in.weight'), G.get('conv_in.bias'))
+            if need_dx:
+                # data gradient of conv_in: ch -> in_channels (rows padded to 4 floats), then NCHW.  Its operand is packed
+                # here, only by the backwards that need it, so the training step keeps its launches
+                with torch.no_grad():
+                    P['conv_in.T'] = ops.pack_weight(m.conv_in.weight, T3D, mode=1, round_tf32=False, out=P.get('conv_in.T'))
+                dxb = View(m._buf('g.x0', (B, H, H, xin.ld)), 0, xin.C)
+                _dgrad_into(m, gview(hv), T3D, P['conv_in.T'], dxb, (B, H, H), xin.C, False)
 
-    # ---- time embedding (M2:293-299) and the per-block temb_proj rows (M2:121)
+    if time_train:
+        _time_bwd(m, top, G, dcond_all)
+    if not need_dx:
+        return None
+    dx = torch.empty((B, dxb.C, H, H), device=dout.device, dtype=torch.float32)
+    call('cd_nhwc_to_nchw_add', C.c_void_p(dxb.addr()), dxb.ld, B, H, H, dxb.C, NULL, ptr(dx), stream())
+    return dx
+
+
+def _time_bwd(m, top, G, dcond_all):
+    """time embedding (M2:293-299) and the per-block temb_proj rows (M2:121); frozen parameters are skipped"""
+    B = top['B']
+    P = m._packed
     d0, d1 = m.temb.dense[0], m.temb.dense[1]
     st, temb, a0, h0, emb = top['st'], top['temb'], top['a0'], top['h0'], top['emb']
     tch = m.temb_ch
     for name, b in m._resblocks():
         off, co = b._cond_off, b.out_channels
+        gw, gb = G.get(name + '.temb_proj.weight'), G.get(name + '.temb_proj.bias')
         # dW[c][k] += sum_b dcond[b][off+c] * st[b][k]
-        call('cd_small_gemm', C.c_void_p(dcond_all.data_ptr() + 4 * off), m._sumC, 1, ptr(st), tch, 0,
-             ptr(G[name + '.temb_proj.weight']), tch, co, tch, B, 1, stream())
-        call('cd_colsum', C.c_void_p(dcond_all.data_ptr() + 4 * off), m._sumC, C.c_int64(B), co, ptr(G[name + '.temb_proj.bias']), stream())
+        if gw is not None:
+            call('cd_small_gemm', C.c_void_p(dcond_all.data_ptr() + 4 * off), m._sumC, 1, ptr(st), tch, 0,
+                 ptr(gw), tch, co, tch, B, 1, stream())
+        if gb is not None:
+            call('cd_colsum', C.c_void_p(dcond_all.data_ptr() + 4 * off), m._sumC, C.c_int64(B), co, ptr(gb), stream())
+    g0w, g0b, g1w, g1b = (G.get('temb.dense.%s' % n) for n in ('0.weight', '0.bias', '1.weight', '1.bias'))
+    if g0w is None and g0b is None and g1w is None and g1b is None:
+        return
     dst = m._buf('g.dst', (B, tch))
     call('cd_small_gemm', ptr(dcond_all), m._sumC, 0, ptr(P['cond.w']), tch, 0, ptr(dst), tch, B, tch, m._sumC, 0, stream())
     dtemb = m._buf('g.dtemb', (B, tch))
     call('cd_swish', ptr(dst), ptr(temb), C.c_int64(B * tch), ptr(dtemb), NULL, stream())
-    call('cd_small_gemm', ptr(dtemb), tch, 1, ptr(a0), tch, 0, ptr(G['temb.dense.1.weight']), tch, tch, tch, B, 1, stream())
-    call('cd_colsum', ptr(dtemb), tch, C.c_int64(B), tch, ptr(G['temb.dense.1.bias']), stream())
+    if g1w is not None:
+        call('cd_small_gemm', ptr(dtemb), tch, 1, ptr(a0), tch, 0, ptr(g1w), tch, tch, tch, B, 1, stream())
+    if g1b is not None:
+        call('cd_colsum', ptr(dtemb), tch, C.c_int64(B), tch, ptr(g1b), stream())
+    if g0w is None and g0b is None:
+        return
     da0 = m._buf('g.da0', (B, tch))
     call('cd_small_gemm', ptr(dtemb), tch, 0, ptr(d1.weight), tch, 0, ptr(da0), tch, B, tch, tch, 0, stream())
     dh0 = m._buf('g.dh0', (B, tch))
     call('cd_swish', ptr(da0), ptr(h0), C.c_int64(B * tch), ptr(dh0), NULL, stream())
-    call('cd_small_gemm', ptr(dh0), tch, 1, ptr(emb), m.ch, 0, ptr(G['temb.dense.0.weight']), m.ch, tch, m.ch, B, 1, stream())
-    call('cd_colsum', ptr(dh0), tch, C.c_int64(B), tch, ptr(G['temb.dense.0.bias']), stream())
+    if g0w is not None:
+        call('cd_small_gemm', ptr(dh0), tch, 1, ptr(emb), m.ch, 0, ptr(g0w), m.ch, tch, m.ch, B, 1, stream())
+    if g0b is not None:
+        call('cd_colsum', ptr(dh0), tch, C.c_int64(B), tch, ptr(g0b), stream())

@@ -139,19 +139,58 @@ class FusedAdamEMA:
         self.m = torch.zeros_like(engine.flat_param)
         self.v = torch.zeros_like(engine.flat_param)
         self.t = 0
+        self._trainable = None      # requires_grad of every parameter, fixed at the first step()
+        self._runs = None           # [(start, end, trainable)]: maximal runs of the flat buffer
 
     def zero_grad(self, set_to_none=False):
         self.engine.flat_grad.zero_()
 
+    def _named_params(self):
+        e = self.engine
+        return list((e.unet if hasattr(e, 'unet') else e.model).named_parameters())
+
+    def _plan_runs(self):
+        """Adam runs over the trainable parameters only (frozen ones get no gradient and no update), in as few launches as the
+        flat layout allows: one per maximal run of trainable slices.  The set is taken at the first step: the one step counter
+        t (Adam's bias correction) is exact only for a fixed set."""
+        named = self._named_params()
+        flags = tuple(p.requires_grad for _, p in named)
+        if self._trainable is None:
+            self._trainable = flags
+            offs = self.engine._offsets
+            total = self.engine.flat_param.numel()
+            spans = sorted((offs[n][0], flag) for (n, _), flag in zip(named, flags))
+            runs = []
+            for i, (start, flag) in enumerate(spans):
+                end = spans[i + 1][0] if i + 1 < len(spans) else total
+                if runs and runs[-1][2] == flag:
+                    runs[-1] = (runs[-1][0], end, flag)
+                else:
+                    runs.append((start, end, flag))
+            self._runs = runs
+        elif flags != self._trainable:
+            n = next(n for (n, _), a, b in zip(named, flags, self._trainable) if a != b)
+            raise ValueError("FusedAdamEMA: parameter %r changed requires_grad after the first step; the trainable set is fixed "
+                             "for the life of the optimizer (create a new one to train a different set)" % n)
+        return self._runs
+
     def step(self, ema_mode=0, ema_beta=0.0, grad_scale=1.0):
         g = self.param_groups[0]
+        runs = self._plan_runs()
         self.t += 1
         e = self.engine
         ema = self.ema_engine.flat_param if (self.ema_engine is not None and ema_mode) else None
-        call('cd_adam_ema_step', ptr(e.flat_param), ptr(e.flat_grad), ptr(self.m), ptr(self.v), ptr(ema),
-             C.c_int64(e.flat_param.numel()), C.c_float(g['lr']), C.c_float(g['betas'][0]), C.c_float(g['betas'][1]),
-             C.c_float(g['eps']), self.t, int(ema_mode) if ema is not None else 0, C.c_float(ema_beta),
-             C.c_float(grad_scale), stream())
+        at = lambda t, off: None if t is None else C.c_void_p(t.data_ptr() + 4 * off)
+        for start, end, trainable in runs:
+            if trainable:
+                call('cd_adam_ema_step', at(e.flat_param, start), at(e.flat_grad, start), at(self.m, start), at(self.v, start),
+                     at(ema, start), C.c_int64(end - start), C.c_float(g['lr']), C.c_float(g['betas'][0]),
+                     C.c_float(g['betas'][1]), C.c_float(g['eps']), self.t, int(ema_mode) if ema is not None else 0,
+                     C.c_float(ema_beta), C.c_float(grad_scale), stream())
+            elif ema is not None:
+                # the EMA covers every parameter (the reference's update_model_average), frozen ones included
+                call('cd_ema_update', at(ema, start), at(e.flat_param, start), C.c_int64(end - start), C.c_float(ema_beta),
+                     int(ema_mode), stream())
         e.mark_weights_dirty()
         if ema is not None:
             self.ema_engine.mark_weights_dirty()

@@ -165,7 +165,7 @@ class Unet(nn.Module):
             if self.time_mlp is not None:
                 raise TypeError("Unet.forward: `time` is required when the network has a time embedding")
             time = torch.zeros(x.shape[0], dtype=torch.int64, device=x.device)
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
             from .autograd import UnetFunction
             return UnetFunction.apply(self, x, time, *self.engine.param_list())
         if self.engine.use_cuda_graph:

@@ -226,7 +226,8 @@ int cd_conv_tc_set_two_ctas(int mask);
 /* ------------------------------------------------------------------------------------------
  * Backward of the HBM-bound pieces (autograd of the reference modules restated as kernels).
  * ------------------------------------------------------------------------------------------ */
-/* LayerNorm (DB:111-121): dh = dLN(dy) (+addend); dg, dbeta accumulated (+=) */
+/* LayerNorm (DB:111-121): dh = dLN(dy) (+addend); dg, dbeta accumulated (+=).  dg = dbeta = NULL (both or neither): dh only,
+ * the same bits, with no parameter reduction (frozen g and b) */
 int cd_layernorm_bwd(const float* dy, int dy_ld, const float* h, int h_ld, const float* stats,
                      const float* g, int64_t npix, int C, const float* addend, int addend_ld,
                      float* dh, int dh_ld, float* dg, float* dbeta, void* stream);
@@ -354,6 +355,9 @@ int cd_transpose_batched(const float* src, int ld, int B, int R, int C, float* d
 /* F.interpolate(scale_factor=2, mode='nearest') on NHWC (M2:47-48) */
 int cd_upsample_nearest2x(const float* x, int x_ld, int B, int H, int W, int C, float* y, int y_ld, void* stream);
 int cd_nhwc_to_nchw(const float* x, int ld, int B, int H, int W, int C, float* out, void* stream);
+/* out = x (NHWC, row stride ld) + add (NCHW, the shape of out) in one pass; add = NULL is cd_nhwc_to_nchw (input gradient of the
+ * networks, with the `x +` term of Unet(residual=True) as the addend) */
+int cd_nhwc_to_nchw_add(const float* x, int ld, int B, int H, int W, int C, const float* add, float* out, void* stream);
 /* get_timestep_embedding -> dense0 -> act -> dense1 (= temb) ; cond_all = Wc act(temb) + bc (all blocks' temb_proj) (M2:6-24,289-294,122).
  * temb ([B][tdim], optional output): when given, the dense layers run one block per sample and the sumC conditioning rows are
  * spread over the whole grid (2 launches); with temb == NULL everything runs in one block per sample (1 launch, slow for large sumC). */
@@ -367,7 +371,8 @@ int cd_ema_update(float* ema, const float* p, int64_t n, float beta, int mode, v
  * Training-mode pieces of the DDPM-style `Model` (Model2.py, "M2"); wired behind COLDDIFF_MODEL_TRAINING=1.
  *   cd_groupnorm_bwd         : backward of GroupNorm(32, eps 1e-6) [+ swish] (M2:32-33,116-125); x is the forward input, cond the
  *                              per-sample channel offset added before the norm (temb_proj row, M2:121); accumulates dgamma / dbeta,
- *                              writes dx and (optionally) dcond[b][c] = sum over pixels of dx
+ *                              writes dx and (optionally) dcond[b][c] = sum over pixels of dx.  dgamma = dbeta = NULL (both or
+ *                              neither): no parameter reduction (frozen gamma and beta), dx and dcond unchanged
  *   cd_dropout               : y = x * keep / (1 - p) with a counter-based mask of (seed, element index) -- the same call with the
  *                              same seed on the gradient is the backward (M2:125; torch's RNG stream is not reproduced)
  *   cd_softmax_bwd_rows      : ds <- s * (ds - sum_j ds*s) * scale for s = softmax(scale * logits) (M2:172-175)
