@@ -46,6 +46,16 @@ __device__ __forceinline__ void load_plane(float* dst, int ldd, const float* __r
   }
 }
 
+// dst[c][r] = src[r][c] (ld S both): thread i reads a float4 of row i % S, so a warp stores 32 consecutive floats of a dst row
+__device__ __forceinline__ void load_plane_transposed(float* dst, const float* __restrict__ src, int S) {
+  const int nv = (S * S) >> 2;
+  for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+    const int r = i % S, c = (i / S) * 4;
+    const float4 v = __ldg(reinterpret_cast<const float4*>(src + r * S + c));
+    dst[(c + 0) * S + r] = v.x; dst[(c + 1) * S + r] = v.y; dst[(c + 2) * S + r] = v.z; dst[(c + 3) * S + r] = v.w;
+  }
+}
+
 __device__ __forceinline__ float block_sum(float v, float* scratch) {
   v = cd_warp_sum(v);
   const int w = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -79,6 +89,9 @@ __device__ __forceinline__ void plane_apply(const float* As, const float* Xs, fl
 
 // smem layout: As[S*S] | Xs[S*ldp] | Yt[S*ldp] | scratch[32]   (Zs aliases Xs after step 1... no: Xs is
 // read only in step 1, Zs written in step 2 -> Zs = Xs)
+// kAdj: the adjoint A^T G A of the same operator (the gradient of A X A^T): A_idx is loaded transposed into As, and the
+// collapse at T-1 comes first -- the adjoint of X -> mean(A X A^T) 11^T is G -> A^T (mean(G) 11^T) A.
+template <bool kAdj>
 __global__ void __launch_bounds__(256)
 blur_apply_kernel(const float* __restrict__ x, float* __restrict__ out, const float* __restrict__ ops,
                   const long long* __restrict__ t, int t_scalar, int S, int T, int collapse_last, int quantize) {
@@ -92,12 +105,22 @@ blur_apply_kernel(const float* __restrict__ x, float* __restrict__ out, const fl
   float* op = out + pl * S * S;
   const int idx = t ? static_cast<int>(t[b]) : t_scalar;
   load_plane(Xs, ldp, xp, S);
-  if (idx >= 0) load_plane(As, S, ops + static_cast<long long>(idx) * S * S, S);
+  if (idx >= 0) {
+    if (kAdj) load_plane_transposed(As, ops + static_cast<long long>(idx) * S * S, S);
+    else load_plane(As, S, ops + static_cast<long long>(idx) * S * S, S);
+  }
   __syncthreads();
-  if (idx >= 0) plane_apply(As, Xs, Yt, Xs, S, ldp);
   float mean = 0.f;
   const bool collapse = collapse_last && idx == T - 1;
-  if (collapse) {
+  if (kAdj && collapse) {
+    float s = 0.f;
+    for (int i = threadIdx.x; i < S * S; i += blockDim.x) s += Xs[(i / S) * ldp + (i % S)];
+    mean = block_sum(s, scratch) / (S * S);
+    for (int i = threadIdx.x; i < S * S; i += blockDim.x) Xs[(i / S) * ldp + (i % S)] = mean;
+    __syncthreads();
+  }
+  if (idx >= 0) plane_apply(As, Xs, Yt, Xs, S, ldp);
+  if (!kAdj && collapse) {
     float s = 0.f;
     for (int i = threadIdx.x; i < S * S; i += blockDim.x) s += Xs[(i / S) * ldp + (i % S)];
     mean = block_sum(s, scratch) / (S * S);
@@ -106,7 +129,7 @@ blur_apply_kernel(const float* __restrict__ x, float* __restrict__ out, const fl
   for (int i = threadIdx.x; i < (S * S) >> 2; i += blockDim.x) {
     const int r = i / per_row, c = (i % per_row) * 4;
     float4 v = *reinterpret_cast<const float4*>(Xs + r * ldp + c);
-    if (collapse) v = make_float4(mean, mean, mean, mean);
+    if (!kAdj && collapse) v = make_float4(mean, mean, mean, mean);
     if (quantize) {
       float* f = reinterpret_cast<float*>(&v);
 #pragma unroll
@@ -214,8 +237,9 @@ __device__ __forceinline__ void strip_for_each(int S, int r0, F f) {
     }
 }
 
-// acc <- this thread's part of the strip of A X A^T (rows and columns outside the plane hold garbage)
-template <int NQ>
+// acc <- this thread's part of the strip of A X A^T (rows and columns outside the plane hold garbage).
+// kAdj: the strip of A^T X A.  Only the operator loads differ: both chunks of A^T are row segments of A, copied 16 bytes at a time.
+template <int NQ, bool kAdj>
 __device__ __forceinline__ void strip_product(const float* __restrict__ A, const float* __restrict__ X, int S, int r0, float* sm,
                                               float (&acc)[NQ][4][4]) {
   constexpr int ldb = strip_ldb<NQ>();
@@ -257,10 +281,18 @@ __device__ __forceinline__ void strip_product(const float* __restrict__ A, const
       cd_cp_async16(rb + kk * ldb + j, X + (v ? static_cast<long long>(k0 + kk) * S + j : 0), v);
     }
     float* ab = aring + (c & 1) * kStripK * kStripR;
-    for (int i = threadIdx.x; i < kStripK * kStripR; i += kStripThreads) {
-      const int r = i / kStripK, kk = i - r * kStripK;          // kk fastest: a warp reads two 64-byte row segments of A
-      const bool v = r0 + r < S && k0 + kk < S;
-      cd_cp_async4(ab + kk * kStripR + r, A + (v ? static_cast<long long>(r0 + r) * S + k0 + kk : 0), v);
+    if (kAdj) {                                                 // aring[kk][r] = A^T[r0 + r][k0 + kk] = A[k0 + kk][r0 + r]
+      for (int i = threadIdx.x; i < kStripK * (kStripR / 4); i += kStripThreads) {
+        const int kk = i / (kStripR / 4), r = (i - kk * (kStripR / 4)) * 4;
+        const bool v = r0 + r < S && k0 + kk < S;              // S % 4 == 0: a float4 is wholly inside or outside
+        cd_cp_async16(ab + kk * kStripR + r, A + (v ? static_cast<long long>(k0 + kk) * S + r0 + r : 0), v);
+      }
+    } else {
+      for (int i = threadIdx.x; i < kStripK * kStripR; i += kStripThreads) {
+        const int r = i / kStripK, kk = i - r * kStripK;          // kk fastest: a warp reads two 64-byte row segments of A
+        const bool v = r0 + r < S && k0 + kk < S;
+        cd_cp_async4(ab + kk * kStripR + r, A + (v ? static_cast<long long>(r0 + r) * S + k0 + kk : 0), v);
+      }
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
@@ -274,14 +306,22 @@ __device__ __forceinline__ void strip_product(const float* __restrict__ A, const
       for (int q = 0; q < NQ; ++q) fma4x4(acc[q], a, *reinterpret_cast<const float4*>(rb + kk * ldb + 128 * q));
     }
   };
-  // phase 2, chunk c: ring[kk][j] = A[j][k0 + kk]
+  // phase 2, chunk c: ring[kk][j] = A[j][k0 + kk]  (kAdj: (A^T)^T = A, ring[kk][j] = A[k0 + kk][j], the layout of the X chunks)
   auto issue2 = [&](int c) {
     const int k0 = c * kStripK;
     float* rb = ring + (c & 1) * kStripK * ldb;
-    for (int i = threadIdx.x; i < kStripK * S; i += kStripThreads) {
-      const int j = i / kStripK, kk = i - j * kStripK;
-      const bool v = k0 + kk < S;
-      cd_cp_async4(rb + kk * ldb + j, A + (v ? static_cast<long long>(j) * S + k0 + kk : 0), v);
+    if (kAdj) {
+      for (int i = threadIdx.x; i < kStripK * per_row; i += kStripThreads) {
+        const int kk = i / per_row, j = (i - kk * per_row) * 4;
+        const bool v = k0 + kk < S;
+        cd_cp_async16(rb + kk * ldb + j, A + (v ? static_cast<long long>(k0 + kk) * S + j : 0), v);
+      }
+    } else {
+      for (int i = threadIdx.x; i < kStripK * S; i += kStripThreads) {
+        const int j = i / kStripK, kk = i - j * kStripK;
+        const bool v = k0 + kk < S;
+        cd_cp_async4(rb + kk * ldb + j, A + (v ? static_cast<long long>(j) * S + k0 + kk : 0), v);
+      }
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
@@ -310,22 +350,28 @@ __device__ __forceinline__ void strip_product(const float* __restrict__ A, const
   run(issue2, compute2);                  // its first barrier orders the Yt writes before any read
 }
 
-// mean(A X A^T) = w^T X w / S^2 with w = A^T 1 (column sums of A): the `discrete` collapse without the strip product
-__device__ __forceinline__ float plane_mean_closed_form(const float* __restrict__ A, const float* __restrict__ X, int S,
-                                                        float* w, float* scratch) {
+// w = A^T 1 (column sums of A)
+__device__ __forceinline__ void column_sums(const float* __restrict__ A, int S, float* w) {
   for (int k = threadIdx.x; k < S; k += blockDim.x) {
     float s = 0.f;
     for (int j = 0; j < S; ++j) s += __ldg(A + static_cast<long long>(j) * S + k);
     w[k] = s;
   }
   __syncthreads();
+}
+
+// mean(A X A^T) = w^T X w / S^2 with w = A^T 1: the `discrete` collapse without the strip product
+__device__ __forceinline__ float plane_mean_closed_form(const float* __restrict__ A, const float* __restrict__ X, int S,
+                                                        float* w, float* scratch) {
+  column_sums(A, S, w);
   float s = 0.f;
   for (int i = threadIdx.x; i < S * S; i += blockDim.x) s = fmaf(w[i / S] * __ldg(X + i), w[i % S], s);
   return block_sum(s, scratch) / (static_cast<float>(S) * S);
 }
 
-// acc <- this thread's part of the strip of D = A_idx X A_idx^T  (idx < 0: X itself; collapse at idx == T-1: the plane mean)
-template <int NQ>
+// acc <- this thread's part of the strip of D = A_idx X A_idx^T  (idx < 0: X itself; collapse at idx == T-1: the plane mean).
+// kAdj: of the adjoint A^T X A; its collapse is A^T (mean(X) 11^T) A = mean(X) w w^T.
+template <int NQ, bool kAdj>
 __device__ __forceinline__ void strip_degrade(const float* __restrict__ ops, const float* __restrict__ X, int idx, int S, int T,
                                               int collapse_last, int r0, float* sm, float (&acc)[NQ][4][4]) {
   if (idx < 0) {
@@ -338,7 +384,25 @@ __device__ __forceinline__ void strip_degrade(const float* __restrict__ ops, con
   const float* A = ops + static_cast<long long>(idx) * S * S;
   if (collapse_last && idx == T - 1) {
     float* w = sm + 2 * kStripK * strip_ldb<NQ>() + 2 * kStripK * kStripR;
-    const float mean = plane_mean_closed_form(A, X, S, w, w + strip_cdiv(S, kStripK) * kStripK * kStripLdy);
+    float* scratch = w + strip_cdiv(S, kStripK) * kStripK * kStripLdy;
+    if (kAdj) {
+      column_sums(A, S, w);
+      float s = 0.f;
+      for (int i = threadIdx.x; i < S * S; i += blockDim.x) s += __ldg(X + i);
+      const float mean = block_sum(s, scratch) / (static_cast<float>(S) * S);
+      const int wi = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+      for (int q = 0; q < NQ; ++q)
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+          for (int b = 0; b < 4; ++b) {              // w has S entries: rows and columns outside the plane get 0
+            const int r = r0 + 4 * wi + a, j = 4 * lane + 128 * q + b;
+            acc[q][a][b] = r < S && j < S ? mean * w[r] * w[j] : 0.f;
+          }
+      return;
+    }
+    const float mean = plane_mean_closed_form(A, X, S, w, scratch);
 #pragma unroll
     for (int q = 0; q < NQ; ++q)
 #pragma unroll
@@ -347,10 +411,11 @@ __device__ __forceinline__ void strip_degrade(const float* __restrict__ ops, con
         for (int b = 0; b < 4; ++b) acc[q][a][b] = mean;
     return;
   }
-  strip_product<NQ>(A, X, S, r0, sm, acc);
+  strip_product<NQ, kAdj>(A, X, S, r0, sm, acc);
 }
 
-template <int NQ>
+// kAdj: the adjoint A^T G A of the same operator (cd_blur_apply_adjoint; quantize is then 0)
+template <int NQ, bool kAdj>
 __global__ void __launch_bounds__(kStripThreads, 1)
 blur_apply_strip_kernel(const float* __restrict__ x, float* __restrict__ out, const float* __restrict__ ops,
                         const long long* __restrict__ t, int t_scalar, int C, int S, int T, int collapse_last, int quantize) {
@@ -362,7 +427,7 @@ blur_apply_strip_kernel(const float* __restrict__ x, float* __restrict__ out, co
   float* op = out + static_cast<long long>(pl) * S * S;
   const int idx = t ? static_cast<int>(t[pl / C]) : t_scalar;
   float acc[NQ][4][4];
-  strip_degrade<NQ>(ops, xp, idx, S, T, collapse_last, r0, sm, acc);
+  strip_degrade<NQ, kAdj>(ops, xp, idx, S, T, collapse_last, r0, sm, acc);
   strip_for_each<NQ>(S, r0, [&](int q, int a, long long o) {
     float f[4] = {acc[q][a][0], acc[q][a][1], acc[q][a][2], acc[q][a][3]};
     if (quantize) {
@@ -391,13 +456,13 @@ blur_step_down_strip_kernel(const float* __restrict__ xt, const float* __restric
   const float* xp = xt + static_cast<long long>(pl) * S * S;
   float* op = out + static_cast<long long>(pl) * S * S;
   float acc[NQ][4][4];
-  strip_degrade<NQ>(ops, xh, t_hi, S, T, collapse_last, r0, sm, acc);
+  strip_degrade<NQ, false>(ops, xh, t_hi, S, T, collapse_last, r0, sm, acc);
   strip_for_each<NQ>(S, r0, [&](int q, int a, long long o) {
     const float4 v = __ldg(reinterpret_cast<const float4*>(xp + o));
     *reinterpret_cast<float4*>(op + o) = make_float4(v.x - acc[q][a][0], v.y - acc[q][a][1], v.z - acc[q][a][2], v.w - acc[q][a][3]);
   });
   __syncthreads();
-  strip_degrade<NQ>(ops, xh, t_lo, S, T, 0, r0, sm, acc);
+  strip_degrade<NQ, false>(ops, xh, t_lo, S, T, 0, r0, sm, acc);
   strip_for_each<NQ>(S, r0, [&](int q, int a, long long o) {
     float4 d = *reinterpret_cast<const float4*>(op + o);
     d.x += acc[q][a][0]; d.y += acc[q][a][1]; d.z += acc[q][a][2]; d.w += acc[q][a][3];
@@ -465,16 +530,16 @@ static int strip_grid(int B, int C, int S, unsigned* grid) {
   return 0;
 }
 
-template <int NQ>
+template <int NQ, bool kAdj>
 static int blur_apply_strips(const float* x, float* out, const float* ops, const int64_t* t, int t_scalar, int B, int C, int S,
                              int T, int collapse_last, int quantize, cudaStream_t stream) {
   unsigned grid = 0;
   if (strip_grid(B, C, S, &grid)) return -1;
   const size_t smem = strip_smem<NQ>(S);
   static size_t attr = 0;
-  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_apply_strip_kernel<NQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
-  blur_apply_strip_kernel<NQ><<<grid, kStripThreads, smem, stream>>>(x, out, ops, reinterpret_cast<const long long*>(t), t_scalar,
-                                                                    C, S, T, collapse_last, quantize);
+  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_apply_strip_kernel<NQ, kAdj>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
+  blur_apply_strip_kernel<NQ, kAdj><<<grid, kStripThreads, smem, stream>>>(x, out, ops, reinterpret_cast<const long long*>(t), t_scalar,
+                                                                          C, S, T, collapse_last, quantize);
   CD_LAUNCH_CHECK();
   return 0;
 }
@@ -493,23 +558,36 @@ static int blur_step_down_strips(const float* xt, const float* xhat, float* out,
 }
 
 // S <= 128: one CTA per plane (blur_apply_kernel / blur_step_down_kernel); 128 < S <= 512: one CTA per row strip
-extern "C" int cd_blur_apply(const float* x, float* out, const float* ops, const int64_t* t, int t_scalar,
-                             int B, int C, int S, int T, int collapse_last, int quantize, void* stream) {
-  CD_REQUIRE(S % 4 == 0 && S >= 4 && S <= 512, "cd_blur_apply: image size %d unsupported (need S%%4==0, 4<=S<=512)", S);
+template <bool kAdj>
+static int blur_apply(const char* name, const float* x, float* out, const float* ops, const int64_t* t, int t_scalar, int B, int C,
+                      int S, int T, int collapse_last, int quantize, cudaStream_t stream) {
+  CD_REQUIRE(S % 4 == 0 && S >= 4 && S <= 512, "%s: image size %d unsupported (need S%%4==0, 4<=S<=512)", name, S);
   if (S > 128) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (S <= 256) return blur_apply_strips<2>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, st);
-    if (S <= 384) return blur_apply_strips<3>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, st);
-    return blur_apply_strips<4>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, st);
+    if (S <= 256) return blur_apply_strips<2, kAdj>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, stream);
+    if (S <= 384) return blur_apply_strips<3, kAdj>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, stream);
+    return blur_apply_strips<4, kAdj>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, stream);
   }
   const size_t smem = blur_smem(S, 2);
   static size_t attr = 0;
-  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
+  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_apply_kernel<kAdj>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
   dim3 grid(C, B);
-  blur_apply_kernel<<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(x, out, ops, reinterpret_cast<const long long*>(t),
-                                                                          t_scalar, S, T, collapse_last, quantize);
+  blur_apply_kernel<kAdj><<<grid, 256, smem, stream>>>(x, out, ops, reinterpret_cast<const long long*>(t), t_scalar, S, T,
+                                                       collapse_last, quantize);
   CD_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int cd_blur_apply(const float* x, float* out, const float* ops, const int64_t* t, int t_scalar,
+                             int B, int C, int S, int T, int collapse_last, int quantize, void* stream) {
+  return blur_apply<false>("cd_blur_apply", x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize,
+                           static_cast<cudaStream_t>(stream));
+}
+
+// the gradient of cd_blur_apply (without its quantize): out = A^T g A per plane, collapse adjoint first at T-1
+extern "C" int cd_blur_apply_adjoint(const float* g, float* out, const float* ops, const int64_t* t, int t_scalar,
+                                     int B, int C, int S, int T, int collapse_last, void* stream) {
+  return blur_apply<true>("cd_blur_apply_adjoint", g, out, ops, t, t_scalar, B, C, S, T, collapse_last, 0,
+                          static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int cd_blur_step_down(const float* xt, const float* xhat, float* out, const float* ops,
@@ -641,6 +719,37 @@ extern "C" int cd_fade_lerp(const float* x1, const float* x2, const int64_t* t, 
   int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   fade_lerp_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x1, x2, reinterpret_cast<const long long*>(t), t_scalar,
                                                                         alphas, one_minus_alphas, C, HW, n, out);
+  CD_LAUNCH_CHECK();
+  return 0;
+}
+
+// -------------------------------------------------------------------------------------------------------------
+// Gradient of the two lerps out = wa[w] x1 + wb[w] x2 (cd_noise_lerp, cd_fade_lerp): both input gradients from one read of g,
+// w = t_b for per-sample scalars (per_pixel = 0) or t_b HW + pixel for per-pixel tables (per_pixel = 1).
+// -------------------------------------------------------------------------------------------------------------
+namespace {
+__global__ void lerp2_adjoint_kernel(const float* __restrict__ g, const long long* __restrict__ t, int t_scalar,
+                                     const float* __restrict__ wa, const float* __restrict__ wb, int C, long long HW, int per_pixel,
+                                     long long n, float* __restrict__ ga, float* __restrict__ gb) {
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long tt = t ? t[i / (HW * C)] : t_scalar;
+    const long long w = per_pixel ? tt * HW + i % HW : tt;
+    const float gv = g[i];
+    if (ga) ga[i] = wa[w] * gv;
+    if (gb) gb[i] = wb[w] * gv;
+  }
+}
+}  // namespace
+
+extern "C" int cd_lerp2_adjoint(const float* g, const int64_t* t, int t_scalar, const float* wa, const float* wb, int B, int C,
+                                int64_t HW, int per_pixel, float* ga, float* gb, void* stream) {
+  CD_REQUIRE(g && wa && wb && (ga || gb) && B >= 0 && C >= 1 && HW >= 0 && (per_pixel == 0 || per_pixel == 1),
+             "cd_lerp2_adjoint: bad arguments");
+  const long long n = static_cast<long long>(B) * C * HW;
+  if (n == 0) return 0;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
+  lerp2_adjoint_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(g, reinterpret_cast<const long long*>(t), t_scalar, wa, wb,
+                                                                            C, HW, per_pixel, n, ga, gb);
   CD_LAUNCH_CHECK();
   return 0;
 }

@@ -12,6 +12,7 @@ from torch import nn
 import torch.nn.functional as F  # noqa: F401  (kept for API familiarity; not used on the hot path)
 
 from ._lib import call, ptr, stream
+from .autograd import BlurDegrade, refuse_grad
 from .degradation import build_blur_operators
 
 
@@ -109,6 +110,18 @@ class GaussianDiffusion(nn.Module):
         with torch.no_grad():
             t = t.to(device=x_start.device, dtype=torch.int64).contiguous()
             return self._apply_op(x_start, -1, per_sample_t=t, quantize=self.discrete)
+
+    def degrade(self, x_start, t):
+        """D(x_start_b, t_b): `q_sample`'s values bit for bit (same kernel), differentiable with respect to x_start, with the
+        gradient A_t^T g A_t.  For reconstruction guidance and for inverting the degradation by gradient descent; q_sample itself
+        stays detached, as the reference's is.  `discrete` (8-bit truncation, zero derivative almost everywhere) raises when a
+        gradient is requested."""
+        if self.discrete:
+            refuse_grad("the `discrete` 8-bit truncation", x_start)
+        x = x_start.contiguous().float()
+        assert x.shape[1:] == (self.channels, self.image_size, self.image_size)
+        t = t.to(device=x.device, dtype=torch.int64).contiguous()
+        return BlurDegrade.apply(x, self._ops_cum, t, -1, self.num_timesteps, self.discrete, self.discrete)
 
     def p_losses(self, x_start, t):
         if self.train_routine == 'Final':

@@ -10,6 +10,7 @@ import torch
 from torch import nn
 
 from ._lib import call, ptr, stream
+from .autograd import MaskDegrade, refuse_grad
 from .deblurring import _LossFn
 from .degradation import gaussian_taps
 
@@ -78,6 +79,16 @@ class GaussianDiffusion(nn.Module):
             rx, ry = _offsets if _offsets is not None else self._offsets(x_start.size(0), x_start.device)
             t = t.to(device=x_start.device, dtype=torch.int64).contiguous()
             return self._fade(x_start, -1, rx, ry, per_sample_t=t, quantize=self.discrete)
+
+    def degrade(self, x_start, t, _offsets=None):
+        """D(x_start_b, t_b) = x_start * mask: `q_sample`'s values bit for bit (same kernel, same per-sample windows of the
+        'Random_*' routines -- pass the same `_offsets`), differentiable with respect to x_start.  `discrete` (8-bit
+        truncation) raises when a gradient is requested."""
+        if self.discrete:
+            refuse_grad("the `discrete` 8-bit truncation", x_start)
+        rx, ry = _offsets if _offsets is not None else self._offsets(x_start.size(0), x_start.device)
+        t = t.to(device=x_start.device, dtype=torch.int64).contiguous()
+        return MaskDegrade.apply(x_start.contiguous().float(), self._masks_cum, t, rx, ry, self.discrete)
 
     def p_losses(self, x_start, t):
         x_fade = self.q_sample(x_start=x_start, t=t)

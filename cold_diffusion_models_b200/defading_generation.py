@@ -11,6 +11,7 @@ import torch
 from torch import nn
 
 from ._lib import call, ptr, stream
+from .autograd import LerpDegrade
 from .deblurring import _LossFn
 from .degradation import gaussian_taps
 
@@ -85,6 +86,17 @@ class GaussianDiffusion(nn.Module):
         """DFGEN:543-548; t: (B,) int64"""
         with torch.no_grad():
             return self._lerp(x_start, x_end, t)
+
+    def degrade(self, x_start, x_end, t):
+        """alphas[t_b] x_start + one_minus_alphas[t_b] x_end per pixel: `q_sample`'s values bit for bit (same kernel),
+        differentiable with respect to both images"""
+        x_start = x_start.contiguous().float(); x_end = x_end.contiguous().float()
+        B, Cc, H, W = x_start.shape
+        assert H == W == self.image_size and x_end.shape == x_start.shape
+        if isinstance(t, int):
+            return LerpDegrade.apply(x_start, x_end, None, t, self.alphas, self.one_minus_alphas, 1)
+        t = t.to(device=x_start.device, dtype=torch.int64).contiguous()
+        return LerpDegrade.apply(x_start, x_end, t, 0, self.alphas, self.one_minus_alphas, 1)
 
     def get_x2_bar_from_xt(self, x1_bar, xt, t):
         # DFGEN:421-425 (API parity; no sampling loop of the reference calls it)

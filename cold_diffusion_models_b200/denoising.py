@@ -9,6 +9,7 @@ import torch
 from torch import nn
 
 from ._lib import call, ptr, stream
+from .autograd import LerpDegrade
 from .deblurring import _LossFn
 
 
@@ -51,6 +52,13 @@ class GaussianDiffusion(nn.Module):
                  ptr(self.sqrt_one_minus_alphas_cumprod), C.c_int64(x_start[0].numel()), C.c_int64(x_start.numel()),
                  ptr(out), stream())
         return out
+
+    def degrade(self, x_start, x_end, t):
+        """sqrt(alpha_bar_t) x_start + sqrt(1 - alpha_bar_t) x_end: `q_sample`'s values bit for bit (same kernel),
+        differentiable with respect to both images"""
+        x_start = x_start.contiguous().float(); x_end = x_end.contiguous().float()
+        t = t.to(device=x_start.device, dtype=torch.int64).contiguous()
+        return LerpDegrade.apply(x_start, x_end, t, 0, self.sqrt_alphas_cumprod, self.sqrt_one_minus_alphas_cumprod, 0)
 
     def get_x2_bar_from_xt(self, x1_bar, xt, t):
         # DN:377-381 (API parity; the sampling loops use the fused cd_noise_step)

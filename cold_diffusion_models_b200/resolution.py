@@ -15,6 +15,7 @@ from torch import nn
 import torch.nn.functional as F
 
 from ._lib import call, ptr, stream
+from .autograd import BlurDegrade
 from .deblurring import _LossFn
 from .degradation import gaussian_taps, blur_matrix
 
@@ -146,6 +147,14 @@ class GaussianDiffusion(nn.Module):
             t = t.to(device=x_start.device, dtype=torch.int64).contiguous()
             t = torch.where(t < 0, t.max().expand_as(t), t).contiguous()
             return self._apply_op(x_start, -1, per_sample_t=t)
+
+    def degrade(self, x_start, t):
+        """D(x_start_b, t_b): `q_sample`'s values bit for bit (same kernel, same level max(t) for the t = -1 rows),
+        differentiable with respect to x_start (gradient A_t^T g A_t with the tabulated resize operators)."""
+        x = x_start.contiguous().float()
+        t = t.to(device=x.device, dtype=torch.int64).contiguous()
+        t = torch.where(t < 0, t.max().expand_as(t), t).contiguous()
+        return BlurDegrade.apply(x, self._ops_cum, t, -1, self.num_timesteps, 0, 0)
 
     def _loss(self, a, b):
         if self.loss_type == 'l1':

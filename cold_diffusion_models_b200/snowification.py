@@ -24,6 +24,7 @@ from torch import nn
 import torch.nn.functional as F
 
 from ._lib import call, ptr, stream
+from .autograd import ChanmixDegrade, refuse_grad
 from .deblurring import _LossFn
 from .degradation import gaussian_taps
 
@@ -263,23 +264,45 @@ class GaussianDiffusion(nn.Module):
         return out
 
     # ---- forward process ------------------------------------------------------------------------------------------
+    @staticmethod
+    def _q_sample_index(t):
+        """the per-row index q_sample degrades to (-1: the row passes through)"""
+        if bool((t == -1).any()):
+            # reference quirk (SN:373-378): row j of the filtered batch is indexed with the UNFILTERED t[j], and a -1
+            # found there selects the last (fully degraded) element
+            keep = t != -1
+            j = torch.cumsum(keep.long(), 0) - 1                       # filtered row number of every kept row
+            tj = t[j.clamp(min=0)]
+            tj = torch.where(tj == -1, torch.max(t).expand_as(tj), tj)
+            t = torch.where(keep, tj, t)
+        return t
+
     def q_sample(self, x_start, t, return_total_blur=False):
         """SN:344-388: rows with t_b == -1 pass through; the others get D(x_start_b, t_b)."""
         with torch.no_grad():
-            t = t.to(x_start.device)
-            if bool((t == -1).any()):
-                # reference quirk (SN:373-378): row j of the filtered batch is indexed with the UNFILTERED t[j], and a -1
-                # found there selects the last (fully degraded) element
-                keep = t != -1
-                j = torch.cumsum(keep.long(), 0) - 1                       # filtered row number of every kept row
-                tj = t[j.clamp(min=0)]
-                tj = torch.where(tj == -1, torch.max(t).expand_as(tj), tj)
-                t = torch.where(keep, tj, t)
+            t = self._q_sample_index(t.to(x_start.device))
             out = self._degrade(x_start, t, 0)
             if return_total_blur:
                 tmax = torch.where(t == -1, t, torch.max(t).expand_as(t))
                 return out, self._degrade(x_start, tmax, 0)
             return out
+
+    def degrade(self, x_start, t):
+        """`q_sample(x_start, t)`'s values bit for bit.  Decolorization (without Lab) is a per-pixel C x C mix M_t and is
+        differentiable with respect to x_start (gradient M_t^T g, the same kernel with the transposed table).  Snow and the
+        Lab decolor path are nonlinear and clipped: they raise when a gradient is requested."""
+        if not isinstance(self.forward_process, DeColorization):
+            refuse_grad("snow (nonlinear and clipped)", x_start)
+            return self.q_sample(x_start, t)
+        if self._lab_decolor():
+            refuse_grad("the Lab decolor path (nonlinear and clipped)", x_start)
+            return self.q_sample(x_start, t)
+        x = x_start.contiguous().float()
+        t = self._q_sample_index(t.to(x.device)).to(dtype=torch.int64).contiguous()
+        mats = self._tab(x.device)[1]
+        if self.__dict__.get('_mats_t', (None,))[0] is not mats:
+            self._mats_t = (mats, mats.transpose(1, 2).contiguous())
+        return ChanmixDegrade.apply(x, mats, self._mats_t[1], t)
 
     def loss_func(self, pred, true):
         if self.loss_type == 'l1':

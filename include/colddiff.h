@@ -271,6 +271,11 @@ int cd_blur_apply(const float* x, float* out, const float* ops, const int64_t* t
                   int B, int C, int S, int T, int collapse_last, int quantize, void* stream);
 int cd_blur_step_down(const float* xt, const float* xhat, float* out, const float* ops,
                       int t_hi, int t_lo, int B, int C, int S, int T, int collapse_last, void* stream);
+/* cd_blur_apply_adjoint: the gradient of cd_blur_apply (without its quantize) with respect to x: out[b,c] = A_{t_b}^T g[b,c] A_{t_b}
+ * (t_b < 0: copy).  With collapse_last, planes at t_b = T-1 first become mean(g) everywhere (the adjoint of the mean-collapse).
+ * Same operator table, shapes, size limits and aliasing rule as cd_blur_apply; A^T is formed in shared memory, not tabulated. */
+int cd_blur_apply_adjoint(const float* g, float* out, const float* ops, const int64_t* t, int t_scalar,
+                          int B, int C, int S, int T, int collapse_last, void* stream);
 
 /* loss (DB:968-971): mode 0 = L1 mean, 1 = L2 mean; writes *loss (device) and dL/dxhat*scale */
 int cd_loss_fwd_bwd(const float* x0, const float* xhat, int64_t n, int mode, float grad_scale,
@@ -297,6 +302,11 @@ int cd_fade_lerp(const float* x1, const float* x2, const int64_t* t, int t_scala
                  const float* one_minus_alphas, int B, int C, int HW, float* out, void* stream);
 int cd_fade_step(const float* img, const float* x1_bar, const float* x2, int t, const float* alphas,
                  const float* one_minus_alphas, int B, int C, int HW, float* out, void* stream);
+/* cd_lerp2_adjoint: the gradients of out = wa[w] x1 + wb[w] x2 (cd_noise_lerp, cd_fade_lerp) from one pass over g [B][C][HW]:
+ * ga = wa[w] g, gb = wb[w] g, with w = t_b (per_pixel = 0: per-sample scalars, cd_noise_lerp) or t_b * HW + pixel (per_pixel = 1:
+ * [T][HW] tables, cd_fade_lerp).  t: int64 [B], or NULL -> t_scalar.  ga or gb may be NULL (that gradient is not written). */
+int cd_lerp2_adjoint(const float* g, const int64_t* t, int t_scalar, const float* wa, const float* wb, int B, int C,
+                     int64_t HW, int per_pixel, float* ga, float* gb, void* stream);
 /* Gaussian-mask fading (defading-diffusion-pytorch/defading_diffusion_pytorch/defading_diffusion_gaussian.py, "DFG"):
  * masks = cumulative products of the fade kernels [T][MS][MS]; rx/ry (optional, int64 [B]) = per-sample window
  * offsets of the 'Random_*' routines (DFG:359-367); index -1 = identity.
