@@ -78,6 +78,15 @@ class AttnBlock(_P):
         self.proj_out = torch.nn.Conv2d(in_channels, in_channels, kernel_size=1)
 
 
+def _weights_loaded(model, incompatible_keys):
+    """load_state_dict copies into the parameters in place, which a captured graph reads on its next replay; with assign=True
+    it replaces them instead, which forward_graphed() sees as moved storage once it re-reads the parameter list.  Either way
+    every pack is rebuilt."""
+    model._version = model._bwd_version = None
+    if getattr(model, '_engine', None) is not None:
+        model._engine._graph_params = None
+
+
 class Model(nn.Module):
     def __init__(self, *, ch, out_ch, ch_mult=(1, 2, 4, 8), num_res_blocks, attn_resolutions, dropout=0.0,
                  resamp_with_conv=True, in_channels, resolution, with_time_emb=True):
@@ -139,13 +148,18 @@ class Model(nn.Module):
         self.conv_out = torch.nn.Conv2d(block_in, out_ch, kernel_size=3, stride=1, padding=1)
         self._bufs, self._packed, self._version = {}, {}, None
         self.conv_impl = CONV_TC
+        # also runs when an enclosing module (GaussianDiffusion, Trainer.load) loads the state dict
+        self.register_load_state_dict_post_hook(_weights_loaded)
 
     # ---------------------------------------------------------------------------------------------------------
     def _apply(self, fn, *a, **k):
         self._bufs, self._packed, self._version = {}, {}, None
+        if getattr(self, '_engine', None) is not None:
+            self._engine.drop_graphs()          # the captured graphs address the buffers and parameters dropped here
         return super()._apply(fn, *a, **k)
 
     def __deepcopy__(self, memo):
+        # the copy (Trainer's EMA model) keeps the CUDA-graph switch (`_cuda_graph`) but gets its own engine, hence its own graphs
         import copy
         new = self.__class__.__new__(self.__class__)
         memo[id(self)] = new
@@ -155,7 +169,8 @@ class Model(nn.Module):
 
     @property
     def engine(self):
-        """flat parameter / gradient buffers for Trainer + FusedAdamEMA (training path, model2_train.py)"""
+        """flat parameter / gradient buffers for Trainer + FusedAdamEMA (training path, model2_train.py), and the CUDA-graph
+        replay of the inference forward (`enable_cuda_graph`)"""
         if getattr(self, '_engine', None) is None:
             from .model2_train import ModelEngine
             self._engine = ModelEngine(self)
@@ -210,12 +225,21 @@ class Model(nn.Module):
             out += [('up.%d.attn.%d' % (i, j), a) for j, a in enumerate(u.attn)]
         return out
 
-    def _prepare(self):
-        ver = tuple(p._version for p in self.parameters())
+    def _prepare(self, params=None):
+        """pack the weights when a parameter changed; `params`: the parameter list, when the caller has it cached"""
+        ver = tuple(p._version for p in (self.parameters() if params is None else params))
         if ver == self._version:
             return
+        # every packed operand is refilled in place (persistent tensors): a captured CUDA graph holds their addresses and reads
+        # the new weights on its next replay
         P = self._packed
         pk = lambda key, w, taps: P.__setitem__(key, ops.pack_weight(w, taps, round_tf32=False, out=P.get(key)))
+        dev = self.conv_in.weight.device
+
+        def persistent(key, shape):
+            if key not in P:
+                P[key] = torch.zeros(shape, device=dev)
+            return P[key]
         with torch.no_grad():
             pk('conv_in', self.conv_in.weight, T3)
             pk('conv_out', self.conv_out.weight, T3)
@@ -223,21 +247,17 @@ class Model(nn.Module):
             for name, b in self._resblocks():
                 pk(name + '.c1', b.conv1.weight, T3)
                 pk(name + '.c2', b.conv2.weight, T3)
-                if hasattr(b, 'nin_shortcut'):
-                    pk(name + '.sc', b.nin_shortcut.weight, T1)
-                    P[name + '.b2s'] = (b.conv2.bias + b.nin_shortcut.bias).contiguous()
-                elif hasattr(b, 'conv_shortcut'):
-                    pk(name + '.sc', b.conv_shortcut.weight, T3)
-                    P[name + '.b2s'] = (b.conv2.bias + b.conv_shortcut.bias).contiguous()
+                sc = getattr(b, 'nin_shortcut', None) or getattr(b, 'conv_shortcut', None)
+                if sc is not None:
+                    pk(name + '.sc', sc.weight, T1 if hasattr(b, 'nin_shortcut') else T3)
+                    torch.add(b.conv2.bias, sc.bias, out=persistent(name + '.b2s', (b.out_channels,)))
                 b._cond_off = off
                 off += b.out_channels
             self._sumC = off
-            wc = torch.zeros(off, self.temb_ch, device=self.conv_in.weight.device)
-            bc = torch.zeros(off, device=self.conv_in.weight.device)
+            wc, bc = persistent('cond.w', (off, self.temb_ch)), persistent('cond.b', (off,))
             for name, b in self._resblocks():
                 wc[b._cond_off:b._cond_off + b.out_channels].copy_(b.temb_proj.weight)
                 bc[b._cond_off:b._cond_off + b.out_channels].copy_(b.temb_proj.bias)
-            P['cond.w'], P['cond.b'] = wc, bc
             for name, a in self._attns():
                 for leaf in ('q', 'k', 'v', 'proj_out'):
                     pk(name + '.' + leaf, getattr(a, leaf).weight, T1)
@@ -310,6 +330,12 @@ class Model(nn.Module):
         if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
             from . import model2_train
             return model2_train.ModelFunction.apply(self, x, t, *self.engine.param_list())
+        if getattr(self, '_cuda_graph', False):         # Model.engine.enable_cuda_graph(True)
+            return self.engine.forward_graphed(x, t)
+        return self._forward(x, t)
+
+    def _forward(self, x, t):
+        """the inference forward: the launches that forward_graphed() captures"""
         assert x.shape[2] == x.shape[3] == self.resolution
         self._prepare()
         P = self._packed
