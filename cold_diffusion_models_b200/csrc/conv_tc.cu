@@ -396,6 +396,11 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constan
 // Epilogue: per 32-channel slice each warpgroup writes out (and out2) of its 128 pixels into SWIZZLE_128B staging slices, and one
 // of its threads stores them with TMA tensor stores (the maps' bounds clip ragged tiles and Cout).  The consumers go on into the
 // next tile's mainloop while the stores drain -- the overlap that the 16 x 8 kernel gets from two CTAs per SM.
+// The epilogue operands come from shared memory: two otherwise idle producer warps, one per consumer warpgroup, copy the tile's
+// bias values there and TMA-load the warpgroup's resid or aux pixels of each slice, in two halves of 64 pixels, into its out2
+// staging slice.  A tile's first slice is loaded during its mainloop, each later half as soon as the previous slice's half has been
+// used, so the epilogue no longer waits on dependent DRAM round trips.  (No engine launch with an operand writes out2; one that
+// does overwrites the operand in place with out2 and frees the halves only once that store has read them.)
 // ---------------------------------------------------------------------------------------------
 constexpr int kR256TH = 16;
 constexpr int kR256BoxBytes = kRowsTW * (kR256TH + 2) * 128;     // 36 KB: one tap column of one chunk
@@ -405,36 +410,80 @@ constexpr int kR256Slice = 128 * 128;                            // staging: 128
 constexpr int kR256Threads = 384;
 constexpr int kR256RegsLow = 40, kR256RegsHigh = 232;          // 128 x 40 + 256 x 232 <= 64 K registers
 
-// channels (col, col + 1) of one row of an epilogue operand, as far as they lie below Cout and `ok` (zeros elsewhere: those outputs
-// are clipped by the store)
-__device__ __forceinline__ float2 ld_pair(const float* row, int col, int Cout, bool ok) {
-  if (ok && col + 1 < Cout) return *reinterpret_cast<const float2*>(row + col);
-  if (ok && col < Cout) return make_float2(row[col], 0.f);
-  return make_float2(0.f, 0.f);
+// Epilogue barriers of one consumer warpgroup: the two operand halves (full, empty) and the bias values (full, empty)
+constexpr int kOpFull = 0, kOpEmpty = 2, kBiasFull = 4, kBiasEmpty = 5, kEpiBars = 6;
+
+// the one epilogue operand of a 16 x 16 launch (resid or GELU' aux; a launch with both is not eligible), nullptr without one
+__host__ __device__ __forceinline__ const float* rows256_operand(const TcParams& p) {
+  return p.resid ? p.resid : (p.act == CD_ACT_GELU_BWD ? p.aux : nullptr);
+}
+
+// Epilogue producer of consumer warpgroup cw (one warp of the producer warpgroup), tile by tile as the consumers walk them: the N
+// tile's BN bias values into sbias (zeros from Cout on), then per 32-channel slice the warpgroup's two halves of 4 x 16 operand
+// pixels, each into its half of the so2 slice.  The map's bounds zero-fill pixels outside the grid and channels from Cout on.
+template <int BN>
+__device__ __forceinline__ void rows256_epilogue_producer(const CUtensorMap& mapE, const TcParams& p, int cw, uint8_t* so2,
+                                                          float* sbias, uint64_t* eb) {
+  const int lane = threadIdx.x & 31;
+  const bool opnd = rows256_operand(p) != nullptr;
+  uint32_t bph = 0, oph = 0;                               // oph: parity bit of each half
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    const int co0 = (tile % p.tiles_co) * BN;
+    int mt = tile / p.tiles_co;
+    const int x0 = (mt % p.tiles_x) * kRowsTW; mt /= p.tiles_x;
+    const int yw = (mt % p.tiles_y) * kR256TH + 8 * cw;
+    const int n = mt / p.tiles_y;
+    if (yw >= p.Hg) continue;                              // the consumers skip this tile's epilogue too
+    if (p.bias) {
+      mbar_wait(&eb[kBiasEmpty], bph ^ 1u);
+      for (int i = lane; i < BN; i += 32) sbias[i] = co0 + i < p.Cout ? p.bias[co0 + i] : 0.f;
+      mbar_arrive(&eb[kBiasFull]);                         // one arrival per lane
+      bph ^= 1u;
+    }
+    if (opnd && lane == 0) {
+      for (int c = 0; c < BN / 32 && co0 + 32 * c < p.Cout; ++c)
+        for (int h = 0; h < 2; ++h) {
+          mbar_wait(&eb[kOpEmpty + h], ((oph >> h) & 1u) ^ 1u);
+          mbar_expect_tx(&eb[kOpFull + h], kR256Slice / 2);
+          tma_load_4d(smem_u32(so2 + h * (kR256Slice / 2)), &mapE, &eb[kOpFull + h], co0 + 32 * c, x0, yw + 4 * h, n);
+          oph ^= 1u << h;
+        }
+    }
+    __syncwarp();
+  }
 }
 
 template <int BN, int ABOXES, int STAGES>
 __global__ void __launch_bounds__(kR256Threads, 1)
 conv_rows256_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
                     const __grid_constant__ CUtensorMap mapB0, const __grid_constant__ CUtensorMap mapB1,
-                    const __grid_constant__ CUtensorMap mapO, const __grid_constant__ CUtensorMap mapO2, const __grid_constant__ TcParams p) {
+                    const __grid_constant__ CUtensorMap mapO, const __grid_constant__ CUtensorMap mapO2,
+                    const __grid_constant__ CUtensorMap mapE, const __grid_constant__ TcParams p) {
   constexpr int kBBytes = BN * 128;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   uint8_t* abox = smem;                                    // ABOXES activation boxes
   uint8_t* wtile = smem + ABOXES * kR256BoxBytes;          // STAGES weight tiles
-  uint8_t* stg = wtile + STAGES * kBBytes;                 // per warpgroup: out slice, out2 slice
+  uint8_t* stg = wtile + STAGES * kBBytes;                 // per warpgroup: out slice, out2 (or operand) slice
   uint64_t* bars = reinterpret_cast<uint64_t*>(stg + 4 * kR256Slice);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
   uint64_t* afull = bars + 2 * STAGES;
   uint64_t* aempty = bars + 2 * STAGES + ABOXES;
-  static_assert(2 * (STAGES + ABOXES) * 8 <= 256, "barrier block is 256 bytes");
+  uint64_t* ebars = bars + 2 * (STAGES + ABOXES);          // kEpiBars per consumer warpgroup
+  float* sbias = reinterpret_cast<float*>(bars + 32);      // after the 256-byte barrier block: BN bias values per warpgroup
+  static_assert(2 * (STAGES + ABOXES) * 8 + 2 * kEpiBars * 8 <= 256, "barrier block is 256 bytes");
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumerWarps); }
     for (int i = 0; i < ABOXES; ++i) { mbar_init(&afull[i], 1); mbar_init(&aempty[i], kConsumerWarps); }
+    for (int w = 0; w < 2; ++w) {
+      uint64_t* eb = ebars + w * kEpiBars;
+      for (int h = 0; h < 2; ++h) { mbar_init(&eb[kOpFull + h], 1); mbar_init(&eb[kOpEmpty + h], kConsumerWarps / 2); }
+      mbar_init(&eb[kBiasFull], 32);
+      mbar_init(&eb[kBiasEmpty], kConsumerWarps / 2);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -443,6 +492,9 @@ conv_rows256_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_cons
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(kR256RegsLow));
     if (warp == 0)
       rows_producer<BN, kR256TH, ABOXES, STAGES>(mapA0, mapA1, mapB0, mapB1, p, abox, wtile, afull, aempty, full_bar, empty_bar);
+    else if (warp <= 2 && (p.bias || rows256_operand(p)))
+      rows256_epilogue_producer<BN>(mapE, p, warp - 1, stg + (warp - 1) * 2 * kR256Slice + kR256Slice, sbias + (warp - 1) * BN,
+                                    ebars + (warp - 1) * kEpiBars);
     return;
   }
   asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(kR256RegsHigh));
@@ -455,10 +507,15 @@ conv_rows256_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_cons
   const bool storer = tid == 0;                            // issues (and waits for) the warpgroup's bulk stores
   uint8_t* so = stg + cw * 2 * kR256Slice;
   uint8_t* so2 = so + kR256Slice;
+  uint64_t* eb = ebars + cw * kEpiBars;
+  const float* sb = sbias + cw * BN;
+  const bool opnd = rows256_operand(p) != nullptr;
   auto release = [&](uint64_t* bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
   auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" :: "r"(1 + cw) : "memory"); };
   float acc[2][BN / 2];
   uint32_t stage = 0, ph = 0, ai = 0, aph = 0;
+  uint32_t bph = 0, oph = 0;                               // parities of the bias barrier and of each operand half
+  bool held = false;                                       // the operand halves hold the last slice's out2 until its store has read them
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     int k = 0;
     uint32_t prev = 0, prev_a = 0;
@@ -499,26 +556,34 @@ conv_rows256_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_cons
     const int yw = (mt % p.tiles_y) * kR256TH + 8 * cw;    // first pixel row of this warpgroup
     const int n = mt / p.tiles_y;
     if (yw >= p.Hg) continue;                              // ragged grid: no pixel of this warpgroup lies inside
-    // local row r = 64 h + rl + 8 e (e: acc[4 j + 2 e], acc[4 j + 2 e + 1]) is pixel (x0 + r % 16, yw + r / 16)
-    long long pix[2][2];
-    bool valid[2][2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int r = 64 * h + rl + 8 * e, gx = x0 + r % kRowsTW, gy = yw + r / kRowsTW;
-        valid[h][e] = gx < p.Wg && gy < p.Hg;
-        pix[h][e] = (static_cast<long long>(n) * p.Hg + gy) * p.Wg + gx;
-      }
+    // local row r = 64 h + rl + 8 e (e: acc[4 j + 2 e], acc[4 j + 2 e + 1]) is pixel (x0 + r % 16, yw + r / 16); pixels outside
+    // the grid and channels from Cout on are zero in the staged operands and clipped by the stores
+    if (p.bias) { mbar_wait(&eb[kBiasFull], bph); bph ^= 1u; }
 #pragma unroll
     for (int c = 0; c < BN / 32; ++c) {
       if (co0 + 32 * c >= p.Cout) break;
       if (storer) bulk_wait_read<0>();                     // the previous stores have read the staging slices
       wg_sync();
+      if (held) { release(&eb[kOpEmpty]); release(&eb[kOpEmpty + 1]); held = false; }
       // epi_pair's arithmetic, one step at a time over the 8 column pairs of each half h of the slice: the branches on the epilogue
-      // operands stay outside the element loops, so the 8 independent chains (and their resid / aux loads) overlap
+      // operands stay outside the element loops, so the 8 independent chains overlap
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
+        // SWIZZLE_128B staging: the 16-byte chunk (8 jj + q2) / 4 of local row rr lands at chunk ^ (rr % 8)
+        auto soff = [&](int e, int jj) {
+          const int rr = 64 * h + rl + 8 * e;
+          return rr * 128 + ((((8 * jj + q2) >> 2) ^ (rr & 7)) << 4) + (q2 & 3) * 4;
+        };
+        // the operand (resid or aux) of this half, staged in so2 at the offsets out2 would take: read it before out2 overwrites it
+        float2 o[2][4];
+        if (opnd) {
+          mbar_wait(&eb[kOpFull + h], (oph >> h) & 1u);
+          oph ^= 1u << h;
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) o[e][jj] = *reinterpret_cast<const float2*>(so2 + soff(e, jj));
+        }
         float2 v[2][4];
 #pragma unroll
         for (int e = 0; e < 2; ++e)
@@ -527,27 +592,17 @@ conv_rows256_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_cons
         if (p.bias) {
 #pragma unroll
           for (int jj = 0; jj < 4; ++jj) {
-            const float2 b = ld_pair(p.bias, co0 + 32 * c + 8 * jj + q2, p.Cout, true);
+            const float2 b = *reinterpret_cast<const float2*>(sb + 32 * c + 8 * jj + q2);
 #pragma unroll
             for (int e = 0; e < 2; ++e) { v[e][jj].x += b.x; v[e][jj].y += b.y; }
           }
         }
         if (p.resid) {
-          float2 r[2][4];
 #pragma unroll
           for (int e = 0; e < 2; ++e)
 #pragma unroll
-            for (int jj = 0; jj < 4; ++jj) r[e][jj] = ld_pair(p.resid + pix[h][e] * p.resid_ld, co0 + 32 * c + 8 * jj + q2, p.Cout, valid[h][e]);
-#pragma unroll
-          for (int e = 0; e < 2; ++e)
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) { v[e][jj].x += r[e][jj].x; v[e][jj].y += r[e][jj].y; }
+            for (int jj = 0; jj < 4; ++jj) { v[e][jj].x += o[e][jj].x; v[e][jj].y += o[e][jj].y; }
         }
-        // SWIZZLE_128B staging: the 16-byte chunk (8 jj + q2) / 4 of local row rr lands at chunk ^ (rr % 8)
-        auto soff = [&](int e, int jj) {
-          const int rr = 64 * h + rl + 8 * e;
-          return rr * 128 + ((((8 * jj + q2) >> 2) ^ (rr & 7)) << 4) + (q2 & 3) * 4;
-        };
         if (p.out2) {
 #pragma unroll
           for (int e = 0; e < 2; ++e)
@@ -560,15 +615,10 @@ conv_rows256_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_cons
 #pragma unroll
             for (int jj = 0; jj < 4; ++jj) { v[e][jj].x = cd_gelu(v[e][jj].x); v[e][jj].y = cd_gelu(v[e][jj].y); }
         } else if (p.act == CD_ACT_GELU_BWD) {
-          float2 a[2][4];
 #pragma unroll
           for (int e = 0; e < 2; ++e)
 #pragma unroll
-            for (int jj = 0; jj < 4; ++jj) a[e][jj] = ld_pair(p.aux + pix[h][e] * p.aux_ld, co0 + 32 * c + 8 * jj + q2, p.Cout, valid[h][e]);
-#pragma unroll
-          for (int e = 0; e < 2; ++e)
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) { v[e][jj].x *= cd_gelu_grad(a[e][jj].x); v[e][jj].y *= cd_gelu_grad(a[e][jj].y); }
+            for (int jj = 0; jj < 4; ++jj) { v[e][jj].x *= cd_gelu_grad(o[e][jj].x); v[e][jj].y *= cd_gelu_grad(o[e][jj].y); }
         }
         if (p.round_tf32) {
 #pragma unroll
@@ -580,6 +630,9 @@ conv_rows256_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_cons
         for (int e = 0; e < 2; ++e)
 #pragma unroll
           for (int jj = 0; jj < 4; ++jj) *reinterpret_cast<float2*>(so + soff(e, jj)) = v[e][jj];
+        // The half may be refilled once every warp's reads of it have completed.  An arrive does not wait for shared-memory loads
+        // still in flight, so it comes after the stores above, which consume every loaded value.
+        if (opnd && !p.out2) release(&eb[kOpEmpty + h]);
       }
       fence_proxy_async();                                 // the staging writes precede the bulk stores' reads
       wg_sync();
@@ -588,7 +641,9 @@ conv_rows256_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_cons
         if (p.out2) tma_store_4d(&mapO2, smem_u32(so2), co0 + 32 * c, x0, yw, n);
         bulk_commit();
       }
+      held = opnd && p.out2;
     }
+    if (p.bias) release(&eb[kBiasEmpty]);
   }
   if (storer) bulk_wait<0>();
 }
@@ -636,16 +691,16 @@ int launch_rows(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
   return launch_persistent<conv_rows_kernel<BN, ABOXES, STAGES, CTAS>, smem, CTAS>(maps, p, st);
 }
 
-// maps: A0, A1, B0, B1, out, out2 (one CTA per SM)
+// maps: A0, A1, B0, B1, out, out2, epilogue operand (one CTA per SM)
 template <int BN, int ABOXES, int STAGES>
 int launch_rows256(const CUtensorMap* maps, const TcParams& p, cudaStream_t st) {
-  constexpr size_t smem = size_t(ABOXES) * kR256BoxBytes + size_t(STAGES) * BN * 128 + 4 * kR256Slice + 1024 + 256;
+  constexpr size_t smem = size_t(ABOXES) * kR256BoxBytes + size_t(STAGES) * BN * 128 + 4 * kR256Slice + 256 + 2 * BN * 4 + 1024;
   static_assert(smem <= 232448, "dynamic shared memory of one CTA (227 KB)");
   constexpr auto kernel = conv_rows256_kernel<BN, ABOXES, STAGES>;
   CD_CUDA(smem_limit_once<kernel>(smem));
   const int sms = cd_num_sms();
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
-  kernel<<<grid, kR256Threads, smem, st>>>(maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], p);
+  kernel<<<grid, kR256Threads, smem, st>>>(maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], maps[6], p);
   CD_LAUNCH_CHECK();
   return 0;
 }
@@ -858,11 +913,12 @@ static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, int mode) {
   // and 17-36 % slower with 64 tiles (16^2, Cout = 256), which stay on the per-tap kernel anyway.  The 3x3 forward + data-gradient
   // convolutions of one micro-batch take 23.5 ms instead of 27.2 ms.
   const int tiles256 = p.tiles_x * cd_cdiv(d->Hg, kR256TH) * p.tiles_n * p.tiles_co;
+  // The 16 x 16 kernel stages at most one epilogue operand per slice, so a launch with both resid and aux takes the 16 x 8 tiles.
   const bool rows256 = (mode == 4 || (by_shape && 4 * tiles256 >= 3 * sms)) && d->oys == 1 && d->oxs == 1 && d->oy0 == 0 &&
-                       d->ox0 == 0 && d->Ho == d->Hg && d->Wo == d->Wg;
+                       d->ox0 == 0 && d->Ho == d->Hg && d->Wo == d->Wg && !(d->resid && d->act == CD_ACT_GELU_BWD);
   if (rows256) { p.TH = kR256TH; p.tiles_y = cd_cdiv(d->Hg, kR256TH); p.total_tiles = tiles256; }
   const CUtensorMapDataType dt = g_tf32_map_dtype ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  CUtensorMap maps[6];
+  CUtensorMap maps[7] = {};
   for (int s = 0; s < 2; ++s) {
     const CdConvSrc& cs = d->s[s < d->nsrc ? s : 0];
     int i = 0;
@@ -888,7 +944,14 @@ static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, int mode) {
         !encode_nhwc(&maps[5], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, o2, o2ld, d->Cout, d->Wg, d->Hg, d->B, 1, 1, 0, 0, kRowsTW,
                      kR256TH / 2, 1, 1, 1, "rows out2"))
       return -1;
-    // three boxes (108 KB), 48 KB of weight tiles and 64 KB of staging slices
+    // resid / aux: half a warpgroup's slice {32 ch, 16, 4, 1} per load, fp32 bits as stored (operands_ok: 16-byte aligned base
+    // and pixel stride)
+    const float* opnd = rows256_operand(p);
+    const int opnd_ld = d->resid ? d->resid_ld : d->aux_ld;
+    if (opnd && !encode_nhwc(&maps[6], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, opnd, opnd_ld, d->Cout, d->Wg, d->Hg, d->B, 1, 1, 0, 0,
+                             kRowsTW, kR256TH / 4, 1, 1, 1, "rows operand"))
+      return -1;
+    // three boxes (108 KB), 48 KB of weight tiles, 64 KB of staging slices and the bias values
     if (BN == 128) return launch_rows256<128, 3, 3>(maps, p, st);
     return launch_rows256<64, 3, 6>(maps, p, st);
   }
