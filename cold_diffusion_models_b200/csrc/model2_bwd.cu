@@ -262,8 +262,10 @@ __device__ __forceinline__ float uniform01(unsigned long long seed, unsigned lon
   h ^= h >> 33; h *= 0xff51afd7ed558ccdull; h ^= h >> 33; h *= 0xc4ceb9fe1a85ec53ull; h ^= h >> 33;
   return static_cast<float>(h >> 40) * (1.f / 16777216.f);
 }
+// seed_ptr: the seed is read from device memory (a CUDA graph replays with the seed staged there before each launch), else `seed`
 __global__ void dropout_kernel(const float* __restrict__ x, int x_ld, long long npix, int C, float p, unsigned long long seed,
-                               float* __restrict__ y, int y_ld) {
+                               const unsigned long long* __restrict__ seed_ptr, float* __restrict__ y, int y_ld) {
+  if (seed_ptr) seed = *seed_ptr;
   const long long n = npix * C;
   const float scale = 1.f / (1.f - p);
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -427,13 +429,26 @@ extern "C" int cd_groupnorm_bwd(const float* x, int x_ld, int B, int64_t HW, int
   return 0;
 }
 
-extern "C" int cd_dropout(const float* x, int x_ld, int64_t npix, int C, float p, uint64_t seed, float* y, int y_ld, void* stream) {
-  CD_REQUIRE(p >= 0.f && p < 1.f, "cd_dropout: p must be in [0, 1)");
+static int dropout_launch(const float* x, int x_ld, int64_t npix, int C, float p, uint64_t seed, const uint64_t* seed_ptr, float* y,
+                          int y_ld, void* stream) {
   const long long n = static_cast<long long>(npix) * C;
   int blocks = cd_cdiv(n, 256); if (blocks > cd_num_sms() * 16) blocks = cd_num_sms() * 16; if (blocks < 1) blocks = 1;
-  dropout_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, x_ld, npix, C, p, seed, y, y_ld);
+  dropout_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, x_ld, npix, C, p, seed,
+                                                                       reinterpret_cast<const unsigned long long*>(seed_ptr), y, y_ld);
   CD_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int cd_dropout(const float* x, int x_ld, int64_t npix, int C, float p, uint64_t seed, float* y, int y_ld, void* stream) {
+  CD_REQUIRE(p >= 0.f && p < 1.f, "cd_dropout: p must be in [0, 1)");
+  return dropout_launch(x, x_ld, npix, C, p, seed, nullptr, y, y_ld, stream);
+}
+
+extern "C" int cd_dropout_seed_dev(const float* x, int x_ld, int64_t npix, int C, float p, const uint64_t* seed, float* y, int y_ld,
+                                   void* stream) {
+  CD_REQUIRE(p >= 0.f && p < 1.f, "cd_dropout_seed_dev: p must be in [0, 1)");
+  CD_REQUIRE(seed != nullptr, "cd_dropout_seed_dev: seed must point to device memory");
+  return dropout_launch(x, x_ld, npix, C, p, 0, seed, y, y_ld, stream);
 }
 
 extern "C" int cd_softmax_bwd_rows(const float* s, float* ds, int ld, int64_t rows, int n, float scale, void* stream) {

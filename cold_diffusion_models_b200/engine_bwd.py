@@ -117,6 +117,12 @@ class BackwardMixin:
                 g.zero_()
                 p.grad = g
 
+    def prepare_training_weights(self):
+        """refill the packed operands of the training forward and backward when a parameter changed (before each replay of a
+        captured training step, whose launches read them)"""
+        self.prepare_weights()
+        self.prepare_weights_bwd()
+
     def _gname(self, prefix, leaf):
         return prefix + '.' + leaf
 

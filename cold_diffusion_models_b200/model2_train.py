@@ -170,6 +170,11 @@ class ModelEngine:
     def param_list(self):
         return list(self.model.parameters())
 
+    def prepare_training_weights(self):
+        """refill the packed operands of the training forward and backward when a parameter changed (before each replay of a
+        captured training step, whose launches read them)"""
+        prepare_bwd(self.model)
+
 
 class ModelFunction(torch.autograd.Function):
     @staticmethod
@@ -299,9 +304,17 @@ def _res_fwd(m, name, b, xv, outv, cond_all, save):
     seed = None
     p = float(b.dropout.p)
     if m.training and p > 0.0:
-        seed = int(torch.randint(0, 2 ** 62, (1,)).item())       # host RNG (torch.manual_seed controls it); mask = f(seed, element index)
-        call('cd_dropout', C.c_void_p(n2.addr()), n2.ld, C.c_int64(B * H * W), cout, C.c_float(p), C.c_uint64(seed),
-             C.c_void_p(n2.addr()), n2.ld, stream())
+        from .train_graph import recording
+        draws = recording()
+        if draws is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())       # host RNG (torch.manual_seed controls it); mask = f(seed, element index)
+            call('cd_dropout', C.c_void_p(n2.addr()), n2.ld, C.c_int64(B * H * W), cout, C.c_float(p), C.c_uint64(seed),
+                 C.c_void_p(n2.addr()), n2.ld, stream())
+        else:
+            # captured training step: the same host draw is made before every replay and staged in this device slot
+            seed = draws.dropout_seed()
+            call('cd_dropout_seed_dev', C.c_void_p(n2.addr()), n2.ld, C.c_int64(B * H * W), cout, C.c_float(p), ptr(seed),
+                 C.c_void_p(n2.addr()), n2.ld, stream())
     if cin != cout:
         taps_sc = T1 if hasattr(b, 'nin_shortcut') else T3
         d = ops.make_conv_desc([(n2, T3, P[name + '.c2'], False), (xv, taps_sc, P[name + '.sc'], False)], outv, (B, H, W),
@@ -330,7 +343,10 @@ def _res_bwd(m, name, b, save, dyv, dx_acc, dcond_all, cond_all, G):
     # ---- through conv2 -> dropout -> swish(GroupNorm2(h1 + cond))
     dn2 = View(m._buf('g.n2.%dx%dx%d' % (H, W, cout), (B, H, W, cout)))
     _dgrad_into(m, dyv, T3D, P[name + '.c2T'], dn2, grid, cout, False)
-    if sv['seed'] is not None:
+    if torch.is_tensor(sv['seed']):
+        call('cd_dropout_seed_dev', C.c_void_p(dn2.addr()), dn2.ld, C.c_int64(B * H * W), cout, C.c_float(sv['p']), ptr(sv['seed']),
+             C.c_void_p(dn2.addr()), dn2.ld, stream())
+    elif sv['seed'] is not None:
         call('cd_dropout', C.c_void_p(dn2.addr()), dn2.ld, C.c_int64(B * H * W), cout, C.c_float(sv['p']), C.c_uint64(sv['seed']),
              C.c_void_p(dn2.addr()), dn2.ld, stream())
     dh1 = View(m._buf('g.h1.%dx%dx%d' % (H, W, cout), (B, H, W, cout)))

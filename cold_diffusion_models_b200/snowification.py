@@ -27,6 +27,7 @@ from ._lib import call, ptr, stream
 from .autograd import ChanmixDegrade, refuse_grad
 from .deblurring import _LossFn
 from .degradation import gaussian_taps
+from .train_graph import recording
 
 
 def _lab_convert(image, to_lab, clip=True):
@@ -166,18 +167,21 @@ class Snow(ForwardProcessBase):
         self._layers = None
         self._dev = None
 
-    def layers(self, dev):
-        """[T][SB][3][H][W] fp32 on `dev` (cd_snow's layout), generated there"""
+    def layers(self, dev, out=None):
+        """[T][SB][3][H][W] fp32 on `dev` (cd_snow's layout), generated there.  `out`: generate into this tensor instead of a
+        new cached one (the persistent buffer a captured training step reads)"""
         dev = torch.device(dev)
-        if self._layers is None or self._layers.device != dev:
+        if out is not None or self._layers is None or self._layers.device != dev:
             ch, m, trim, h = self._geom
             T, nsb = self._vertical.shape
             noise, thres, taps, vert = (t.to(dev) for t in (self._noise, self._thres, self._taps, self._vertical))
             base = torch.empty((nsb, h, h), dtype=torch.float32, device=dev)
-            out = torch.empty((T, nsb, 3, h, h), dtype=torch.float32, device=dev)
+            dst = torch.empty((T, nsb, 3, h, h), dtype=torch.float32, device=dev) if out is None else out
             call('cd_snow_layers', ptr(noise), nsb, ch, m, trim, h, ptr(thres), ptr(taps), int(taps.shape[1]), ptr(vert), T,
-                 ptr(base), ptr(out), stream())
-            self._layers = out
+                 ptr(base), ptr(dst), stream())
+            if out is not None:
+                return out
+            self._layers = dst
         return self._layers
 
     # the reference's attributes (FP:305-306, 349-350: lists of CPU tensors), materialised on request
@@ -267,7 +271,8 @@ class GaussianDiffusion(nn.Module):
     @staticmethod
     def _q_sample_index(t):
         """the per-row index q_sample degrades to (-1: the row passes through)"""
-        if bool((t == -1).any()):
+        # a captured training step runs the body unconditionally (no host sync): it maps t to itself when no row is -1
+        if recording() is not None or bool((t == -1).any()):
             # reference quirk (SN:373-378): row j of the filtered batch is indexed with the UNFILTERED t[j], and a -1
             # found there selects the last (fully degraded) element
             keep = t != -1
@@ -304,6 +309,23 @@ class GaussianDiffusion(nn.Module):
             self._mats_t = (mats, mats.transpose(1, 2).contiguous())
         return ChanmixDegrade.apply(x, mats, self._mats_t[1], t)
 
+    def _stage_random_snow(self, draws, dev):
+        """captured training step: reset_parameters() redraws the snow layers on the host, which a graph cannot do.  The draws
+        and the layer generation run before every replay (`draws.stage()`), into a buffer that lives with the graph; the
+        captured cd_snow reads it through the tables set here."""
+        fp = self.forward_process
+        h = fp.image_size[0]
+        nsb = fp._vertical.shape[1]
+        layers = draws.buffer((self.num_timesteps, nsb, 3, h, h))
+        br = draws.buffer(tuple(fp.br_t.shape), init=fp.br_t)
+
+        def regenerate():
+            fp.reset_parameters()
+            fp.layers(dev, out=layers)
+        draws.host_call(regenerate)
+        self._tables = (dev, layers, br)
+        fp._dev = dev
+
     def loss_func(self, pred, true):
         if self.loss_type == 'l1':
             return _LossFn.apply(pred, true, 0)
@@ -317,7 +339,11 @@ class GaussianDiffusion(nn.Module):
         return self.denoise_fn(img, t)
 
     def p_losses(self, x_start, t, t_pred=None):
-        self.forward_process.reset_parameters()
+        draws = recording()
+        if draws is None:
+            self.forward_process.reset_parameters()
+        elif isinstance(self.forward_process, Snow) and self.forward_process.random_snow:
+            self._stage_random_snow(draws, x_start.device)
         if self.train_routine == 'Final':
             x_blur = self.q_sample(x_start=x_start, t=t)
             return self.loss_func(x_start, self.denoise_fn(x_blur, t))

@@ -342,11 +342,60 @@ class Trainer(EvaluationMixin, object):
         """-> (xt, direct_recons, recon) of the EMA model every `save_and_sample_every` steps (DB:1210)"""
         return _unwrap(self.ema_model).sample(batch_size=self.batch_size, img=og_img)
 
+    # ---- CUDA-graph training step -----------------------------------------------------------------------
+    _step_graphs = None         # {(micro-batch shapes, A, merged): train_graph.StepGraph} while the switch is on, else None
+    _graph_ptrs = None          # engine and parameter addresses the graphs were captured with
+
+    def enable_cuda_graph(self, flag=True):
+        """replay the forward + backward of every optimizer step's micro-batches from one captured CUDA graph (off by default).
+        It computes what the eager step computes: the host-side random draws (the `Model`'s dropout seeds, `random_snow`'s snow
+        layers) are made before each replay in eager order, and the torch CUDA generator advances as the eager launches
+        would advance it.  One graph per (micro-batch shapes, gradient_accumulate_every, merge_micro_batches()); parameters
+        that move (`.to()`, `load_state_dict(assign=True)`) trigger a new capture, `load()` does not.  False drops the graphs
+        and returns to eager launches.  Single process only: the multi-GPU step all-reduces gradient ranges from a host
+        callback during the backward, which a replay cannot run."""
+        if flag and self._world > 1:
+            raise ValueError("Trainer.enable_cuda_graph: CUDA-graph training runs in a single process; this trainer has a "
+                             "process group of world size %d" % self._world)
+        self._step_graphs = {} if flag else None
+        self._graph_ptrs = None
+
+    def _graphed_accumulate(self, ds):
+        from . import train_graph
+        A = self.gradient_accumulate_every
+        merged = A > 1 and merge_micro_batches() and all(torch.is_tensor(d) for d in ds) and len({tuple(d.shape) for d in ds}) == 1
+        shapes = tuple(tuple(tuple(x.shape) for x in d) if isinstance(d, (tuple, list)) else tuple(d.shape) for d in ds)
+        eng = self._unet.engine
+        ptrs = (id(eng),) + tuple(p.data_ptr() for p in self._unet.parameters())
+        if ptrs != self._graph_ptrs:
+            self._step_graphs, self._graph_ptrs = {}, ptrs
+        key = (shapes, A, merged)
+        g = self._step_graphs.get(key)
+        if g is None:
+            g = self._step_graphs[key] = train_graph.capture(self, ds)
+        eng.prepare_training_weights()           # the captured launches read the packs: refill them after an optimizer step
+        return g.replay(ds), 1.0
+
     def train_step(self, batches=None):
         """one optimizer step = gradient_accumulate_every micro-batches (DB:1188-1204). Returns mean loss (tensor)."""
-        u_loss = None
         A = self.gradient_accumulate_every
         ds = [batches[i] if batches is not None else self._next() for i in range(A)]
+        if self._step_graphs is not None:
+            u_loss, scale = self._graphed_accumulate(ds)
+        else:
+            u_loss, scale = self._accumulate(ds)
+        ema_mode = 0
+        if self.step % self.update_ema_every == 0:
+            ema_mode = 1 if self.step < self.step_start_ema else 2
+        self.opt.step(ema_mode=ema_mode, ema_beta=self.ema_decay, grad_scale=scale)
+        self.opt.zero_grad()
+        return u_loss / self.gradient_accumulate_every
+
+    def _accumulate(self, ds):
+        """forward + backward of the micro-batches `ds`, gradients accumulated into the flat buffer (and all-reduced across
+        replicas) -> (summed loss, gradient scale of the optimizer step)"""
+        u_loss = None
+        A = self.gradient_accumulate_every
         if (A > 1 and merge_micro_batches() and all(torch.is_tensor(d) for d in ds) and len({tuple(d.shape) for d in ds}) == 1):
             # one pass over the concatenated micro-batches: mean over A * B samples == sum_i mean_i / A
             d = torch.cat([d.cuda(non_blocking=True) for d in ds], dim=0)
@@ -382,12 +431,7 @@ class Trainer(EvaluationMixin, object):
                 w.wait()
         else:
             scale = allreduce_mean_(eng.flat_grad, self._world)            # one NCCL all-reduce per optimizer step
-        ema_mode = 0
-        if self.step % self.update_ema_every == 0:
-            ema_mode = 1 if self.step < self.step_start_ema else 2
-        self.opt.step(ema_mode=ema_mode, ema_beta=self.ema_decay, grad_scale=scale)
-        self.opt.zero_grad()
-        return u_loss / self.gradient_accumulate_every
+        return u_loss, scale
 
     def train(self):
         acc_loss = 0

@@ -385,6 +385,9 @@ int cd_ema_update(float* ema, const float* p, int64_t n, float beta, int mode, v
  *                              neither): no parameter reduction (frozen gamma and beta), dx and dcond unchanged
  *   cd_dropout               : y = x * keep / (1 - p) with a counter-based mask of (seed, element index) -- the same call with the
  *                              same seed on the gradient is the backward (M2:125; torch's RNG stream is not reproduced)
+ *   cd_dropout_seed_dev      : cd_dropout with the seed read from device memory (*seed) when the kernel runs: the same mask
+ *                              function, so the masks are bit-identical to cd_dropout's for the same seed value.  A captured
+ *                              CUDA graph keeps the pointer, and a new seed staged there before each replay gives a new mask
  *   cd_softmax_bwd_rows      : ds <- s * (ds - sum_j ds*s) * scale for s = softmax(scale * logits) (M2:172-175)
  *   cd_upsample_nearest2x_bwd: sum of the four children (M2:47-48)
  *   cd_swish                 : act_out = swish(pre) and / or y = dy * swish'(pre) (M2:27-29)
@@ -394,6 +397,8 @@ int cd_groupnorm_bwd(const float* x, int x_ld, int B, int64_t HW, int C, int gro
                      const float* gamma, const float* beta, float eps, int swish, const float* dy, int dy_ld,
                      float* dx, int dx_ld, float* dgamma, float* dbeta, float* dcond, int dcond_ld, void* stream);
 int cd_dropout(const float* x, int x_ld, int64_t npix, int C, float p, uint64_t seed, float* y, int y_ld, void* stream);
+int cd_dropout_seed_dev(const float* x, int x_ld, int64_t npix, int C, float p, const uint64_t* seed, float* y, int y_ld,
+                        void* stream);
 int cd_softmax_bwd_rows(const float* s, float* ds, int ld, int64_t rows, int n, float scale, void* stream);
 int cd_upsample_nearest2x_bwd(const float* dy, int dy_ld, int B, int H, int W, int C, float* dx, int dx_ld, void* stream);
 int cd_swish(const float* dy, const float* pre, int64_t n, float* y, float* act_out, void* stream);
