@@ -16,6 +16,7 @@ import torch
 from . import ops
 from .ops import View, CONV_TC, CONV_SIMT, ACT_NONE, ACT_GELU
 from ._lib import call, ptr, stream
+from .graphs import GraphedForward
 
 T3 = ops.taps_conv(3, 1)
 T1 = ops.taps_conv(1, 0)
@@ -71,7 +72,7 @@ class AttnSpec:
         self.dim = self.norm.g.shape[1]
 
 
-class UnetEngine(_BackwardHolder):
+class UnetEngine(_BackwardHolder, GraphedForward):
     def __init__(self, unet):
         self.unet = unet
         self.dev = next(unet.parameters()).device
@@ -118,6 +119,7 @@ class UnetEngine(_BackwardHolder):
             if isinstance(mod, torch.nn.Conv2d) and not isinstance(mod, torch.nn.ConvTranspose2d) and mod.groups == 1:
                 self.dense_convs[mn + '.weight'] = tuple(mod.weight.shape)
         self._pname = {id(p): n for n, p in unet.named_parameters()}
+        self._init_graphs(unet, self.forward, self.prepare_weights)        # CUDA-graph replay (enable_cuda_graph)
 
     # ------------------------------------------------------------------------------------------
     _epoch = 0            # bumped by every in-place parameter update that bypasses torch's version counters
@@ -142,8 +144,8 @@ class UnetEngine(_BackwardHolder):
             self._bufs[key] = t
         return t
 
-    def _params_version(self):
-        return tuple(p._version for p in self.unet.parameters())
+    def _params_version(self, params=None):
+        return tuple(p._version for p in (self.unet.parameters() if params is None else params))
 
     @staticmethod
     def packed_view(w):
@@ -200,10 +202,11 @@ class UnetEngine(_BackwardHolder):
         b.clear()
         return b
 
-    def prepare_weights(self, force=False):
-        """(re)pack reference-layout parameters into kernel layouts when they changed."""
-        ver = self._params_version()
-        if not (force or self._dirty or ver != self._version):
+    def prepare_weights(self, params=None):
+        """(re)pack reference-layout parameters into kernel layouts when they changed; `params`: the parameter list, when the
+        caller has it cached"""
+        ver = self._params_version(params)
+        if not (self._dirty or ver != self._version):
             return
         P = self._packed
         batch = self._repack_batch('pack_fwd', 'pack')
@@ -377,42 +380,6 @@ class UnetEngine(_BackwardHolder):
         self._conv(do, n >= 128)
         if save is not None:
             save[spec.name] = dict(x=xv, xn=View(xn), qkv=qkv, kmax=kmax, ksum=ksum, ctx=ctx, weff=weff, stats=stats, out=outv)
-
-    # ------------------------------------------------------------------------------------------
-    # CUDA-graph replay of the inference forward (sampling loops call R(x_t, t) hundreds of times with identical shapes:
-    # ~150 kernel launches collapse into one graph launch; matters when the batch is small and the step is launch-bound)
-    # ------------------------------------------------------------------------------------------
-    use_cuda_graph = False
-    _graphs = None
-
-    def enable_cuda_graph(self, flag=True):
-        self.use_cuda_graph = bool(flag)
-        self._graphs = {}
-
-    def forward_graphed(self, x, time):
-        # the packs write into persistent buffers, so a captured graph stays valid across weight updates: repack before
-        # every replay (no-op when nothing changed) instead of keying the graph on the weights
-        self.prepare_weights()
-        key = tuple(x.shape)
-        g = self._graphs.get(key)
-        if g is None:
-            sx = x.contiguous().float().clone()
-            st = time.to(device=x.device, dtype=torch.int64).contiguous().clone()
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):                      # warm-up outside capture: allocates every workspace
-                for _ in range(2):
-                    self.forward(sx, st)
-            torch.cuda.current_stream().wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                so = self.forward(sx, st)
-            g = self._graphs[key] = (graph, sx, st, so)
-        graph, sx, st, so = g
-        sx.copy_(x)
-        st.copy_(time)
-        graph.replay()
-        return so.clone()
 
     def forward(self, x, time, save=None, out=None):
         """x (B,C,H,W) NCHW fp32 cuda, time (B,) int64 -> (B,out_dim,H,W) NCHW."""

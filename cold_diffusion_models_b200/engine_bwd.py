@@ -101,8 +101,7 @@ class BackwardMixin:
                 v.copy_(p.data)
                 p.data = v
         self._packed = {}              # operands that aliased the old parameter storage
-        if getattr(self, '_graphs', None):
-            self._graphs = {}
+        self.drop_graphs()
         self.mark_weights_dirty()
 
     def attach_grads(self):

@@ -23,6 +23,7 @@ from ._lib import call, ptr, stream
 from .engine_bwd import flat_offsets
 from .autograd import check_first_order, trainable_names, once_differentiable
 from .model2 import T1, T3, TDOWN
+from .graphs import GraphedForward
 
 NULL = C.c_void_p(0)
 T3D = ops.taps_conv_dgrad(3, 1)
@@ -40,21 +41,7 @@ def taps_down_dgrad(py, px):
     return [(ky, kx, dy, dx) for (ky, dy) in ys for (kx, dx) in xs]
 
 
-_CAPTURE_STREAMS = {}
-
-
-def _capture_stream(device):
-    """the one stream per device on which every Model graph is warmed up and captured.  The split GroupNorm (planes above 128²)
-    keeps its partials in a buffer cached per (device, stream) that cannot grow during a capture: the warm-up on this same
-    stream grows it to the shape first."""
-    idx = device.index if device.index is not None else torch.cuda.current_device()
-    s = _CAPTURE_STREAMS.get(idx)
-    if s is None:
-        s = _CAPTURE_STREAMS[idx] = torch.cuda.Stream(device=idx)
-    return s
-
-
-class ModelEngine:
+class ModelEngine(GraphedForward):
     """what Trainer / FusedAdamEMA need from a network: flat parameter and gradient buffers with 16-byte aligned slices; and the
     CUDA-graph replay of the inference forward."""
 
@@ -62,66 +49,7 @@ class ModelEngine:
         self.model = model
         self.flat_grad = self.flat_param = None
         self.G = {}
-        self._graphs, self._graph_params, self._graph_ptrs = {}, None, None
-
-    # ---- CUDA-graph replay of the inference forward ---------------------------------------------------------------------
-    # A sampling loop calls R(x_t, t) T times with identical shapes; replaying the ~200 launches of one forward as one graph
-    # takes the Python schedule off the critical path.  The switch is stored on the model, so a deep copy (the EMA model)
-    # keeps it; the graphs are per engine.
-    @property
-    def use_cuda_graph(self):
-        return getattr(self.model, '_cuda_graph', False)
-
-    def enable_cuda_graph(self, flag=True):
-        self.model._cuda_graph = bool(flag)
-        self.drop_graphs()
-
-    def drop_graphs(self):
-        """forget every captured graph: parameter storage or workspaces moved, and the graphs hold their old addresses"""
-        self._graphs, self._graph_params, self._graph_ptrs = {}, None, None
-
-    def forward_graphed(self, x, t):
-        """the inference forward, replayed from one graph per input shape (B, C, H, W); returns a clone of the graph's output"""
-        m = self.model
-        # the parameter list is cached (two walks of the module tree were most of a replay's host time); it is rebuilt after
-        # load_state_dict, which may replace the Parameter objects (assign=True), and after drop_graphs()
-        if self._graph_params is None:
-            self._graph_params = list(m.parameters())
-        # biases and GroupNorm affines are read straight from the parameters: if any parameter was rebound since the capture
-        # (flatten_params, load_state_dict(assign=True), p.data = ...), the graphs hold stale addresses, and the new storage
-        # has its own version counter: repack and capture again
-        ptrs = tuple(p.data_ptr() for p in self._graph_params)
-        if ptrs != self._graph_ptrs:
-            self._graphs, self._graph_ptrs = {}, ptrs
-            m._version = None
-        # the packs refill persistent tensors, so a graph stays valid across weight updates: repack before every replay
-        # (a no-op when no parameter changed)
-        m._prepare(self._graph_params)
-        key = tuple(x.shape)
-        g = self._graphs.get(key)
-        if g is None:
-            g = self._graphs[key] = self._capture(x, t)
-        graph, sx, st, so = g
-        sx.copy_(x)
-        st.copy_(t)
-        graph.replay()
-        return so.clone()
-
-    def _capture(self, x, t):
-        m = self.model
-        sx = torch.empty(x.shape, device=x.device, dtype=torch.float32)
-        sx.copy_(x)
-        st = torch.empty((x.shape[0],), device=x.device, dtype=torch.int64)
-        st.copy_(t)
-        cs = _capture_stream(x.device)
-        cs.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(cs):             # warm-up outside the capture: allocates every workspace
-            m._forward(sx, st)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=cs):
-            so = m._forward(sx, st)
-        torch.cuda.current_stream().wait_stream(cs)
-        return graph, sx, st, so
+        self._init_graphs(model, model._forward, model._prepare)
 
     @property
     def dev(self):

@@ -15,7 +15,7 @@ at every replay (graph-safe Philox), as the eager launches would.
 import numpy as np
 import torch
 
-from .model2_train import _capture_stream
+from . import graphs
 
 _RECORDING = None
 
@@ -103,19 +103,15 @@ def capture(trainer, ds):
     grad0 = eng.flat_grad.clone()
     rng = (torch.cuda.get_rng_state(dev), torch.get_rng_state(), np.random.get_state())
     draws = HostDraws(dev)
-    cs = _capture_stream(dev)           # the split GroupNorm's workspace is per stream: warm up where the capture runs
-    cs.wait_stream(torch.cuda.current_stream())
+
+    def step():
+        draws.reset()
+        return trainer._accumulate(statics)[0]
     try:
         _RECORDING = draws
-        with torch.cuda.stream(cs):
-            trainer._accumulate(statics)
-        draws.reset()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=cs):
-            loss, _ = trainer._accumulate(statics)
+        graph, loss = graphs.capture(step, dev)
     finally:
         _RECORDING = None
-    torch.cuda.current_stream().wait_stream(cs)
     eng.flat_grad.copy_(grad0)
     torch.cuda.set_rng_state(rng[0], dev)
     torch.set_rng_state(rng[1])

@@ -21,6 +21,7 @@ from torch.utils import data
 
 from ._lib import call, ptr, stream
 from .evaluation import EvaluationMixin, SnowEvaluationMixin
+from .graphs import GraphCache
 
 
 def cycle(dl):
@@ -343,8 +344,7 @@ class Trainer(EvaluationMixin, object):
         return _unwrap(self.ema_model).sample(batch_size=self.batch_size, img=og_img)
 
     # ---- CUDA-graph training step -----------------------------------------------------------------------
-    _step_graphs = None         # {(micro-batch shapes, A, merged): train_graph.StepGraph} while the switch is on, else None
-    _graph_ptrs = None          # engine and parameter addresses the graphs were captured with
+    _step_graphs = None         # {(micro-batch shapes, A, merged): train_graph.StepGraph} (a GraphCache) while the switch is on
 
     def enable_cuda_graph(self, flag=True):
         """replay the forward + backward of every optimizer step's micro-batches from one captured CUDA graph (off by default).
@@ -357,8 +357,7 @@ class Trainer(EvaluationMixin, object):
         if flag and self._world > 1:
             raise ValueError("Trainer.enable_cuda_graph: CUDA-graph training runs in a single process; this trainer has a "
                              "process group of world size %d" % self._world)
-        self._step_graphs = {} if flag else None
-        self._graph_ptrs = None
+        self._step_graphs = GraphCache() if flag else None
 
     def _graphed_accumulate(self, ds):
         from . import train_graph
@@ -367,12 +366,7 @@ class Trainer(EvaluationMixin, object):
         shapes = tuple(tuple(tuple(x.shape) for x in d) if isinstance(d, (tuple, list)) else tuple(d.shape) for d in ds)
         eng = self._unet.engine
         ptrs = (id(eng),) + tuple(p.data_ptr() for p in self._unet.parameters())
-        if ptrs != self._graph_ptrs:
-            self._step_graphs, self._graph_ptrs = {}, ptrs
-        key = (shapes, A, merged)
-        g = self._step_graphs.get(key)
-        if g is None:
-            g = self._step_graphs[key] = train_graph.capture(self, ds)
+        g = self._step_graphs.lookup((shapes, A, merged), ptrs, lambda: train_graph.capture(self, ds))
         eng.prepare_training_weights()           # the captured launches read the packs: refill them after an optimizer step
         return g.replay(ds), 1.0
 

@@ -77,6 +77,15 @@ class SinusoidalPosEmb(_Params):
         self.dim = dim
 
 
+def _weights_loaded(unet, incompatible_keys):
+    """load_state_dict copies into the parameters in place, which a captured graph reads on its next replay; with assign=True
+    it replaces them instead, which forward_graphed() sees as moved storage once it re-reads the parameter list.  Either way
+    every pack is rebuilt."""
+    if unet._engine is not None:
+        unet._engine.mark_weights_dirty()
+        unet._engine._graph_params = None
+
+
 def Upsample(dim):
     return nn.ConvTranspose2d(dim, dim, 4, 2, 1)
 
@@ -128,6 +137,8 @@ class Unet(nn.Module):
         out_dim = out_dim if exists(out_dim) else channels
         self.final_conv = nn.Sequential(ConvNextBlock(dim, dim), nn.Conv2d(dim, out_dim, 1))
         self._engine = None
+        # also runs when an enclosing module (GaussianDiffusion, Trainer.load) loads the state dict
+        self.register_load_state_dict_post_hook(_weights_loaded)
 
     # -- engine plumbing -------------------------------------------------------------------------
     @property
@@ -137,7 +148,8 @@ class Unet(nn.Module):
         return self._engine
 
     def __deepcopy__(self, memo):
-        # the engine (packed weights, workspaces) is per-instance device state: never cloned (Trainer's EMA copy)
+        # the engine (packed weights, workspaces, graphs) is per-instance device state: never cloned; the copy (Trainer's EMA
+        # model) keeps the CUDA-graph switch (`_cuda_graph`) and captures its own graphs
         import copy
         new = self.__class__.__new__(self.__class__)
         memo[id(self)] = new
@@ -146,14 +158,8 @@ class Unet(nn.Module):
         return new
 
     def _apply(self, fn, *a, **k):
-        self._engine = None                     # parameters moved/cast: rebuild packed weights lazily
+        self._engine = None                     # parameters moved/cast: rebuild packed weights and graphs lazily
         return super()._apply(fn, *a, **k)
-
-    def load_state_dict(self, state_dict, *a, **k):
-        r = super().load_state_dict(state_dict, *a, **k)
-        if self._engine is not None:
-            self._engine.mark_weights_dirty()
-        return r
 
     def forward(self, x, time=None):
         """x: (B, C, H, W) fp32 NCHW on a CUDA device, time: (B,) int64  ->  (B, out_dim, H, W)   (DB:256-282).
@@ -168,6 +174,6 @@ class Unet(nn.Module):
         if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
             from .autograd import UnetFunction
             return UnetFunction.apply(self, x, time, *self.engine.param_list())
-        if self.engine.use_cuda_graph:
+        if getattr(self, '_cuda_graph', False):         # Unet.engine.enable_cuda_graph(True)
             return self.engine.forward_graphed(x, time)
         return self.engine.forward(x, time)

@@ -274,6 +274,24 @@ def test_cuda_graph_replay_of_the_sampling_forward(small):
         assert torch.equal(a, b)          # same kernels on the same values: the forward is deterministic
 
 
+def test_cuda_graph_captures_again_after_load_state_dict_assign(small):
+    """load_state_dict(assign=True) replaces the Parameter objects, whose old storage the graph captured before reads: the next
+    call captures again, and its replay equals the eager forward bit for bit"""
+    g, sd, _ = small
+    u = make_unet(32, (1, 2), 3, sd)
+    x, t = g['x'].cuda(), g['t'].cuda()
+    u.engine.enable_cuda_graph(True)
+    with torch.no_grad():
+        y0 = u(x, t)
+        g0 = u.engine._graphs[tuple(x.shape)][0]
+        u.load_state_dict({k: (v * 0.5).cuda() for k, v in sd.items()}, assign=True)
+        graphed = u(x, t)
+        assert u.engine._graphs[tuple(x.shape)][0] is not g0
+        u.engine.enable_cuda_graph(False)
+        eager = u(x, t)
+    assert torch.equal(graphed, eager) and not torch.equal(graphed, y0)
+
+
 def test_all_sample_gen_sample_consistency(small):
     """all_sample (DB:609-689) walks the same trajectory as sample (DB:393-455); gen_sample with noise_level 0 equals sample."""
     import cold_diffusion_models_b200 as cdm
