@@ -914,8 +914,12 @@ static int conv_fwd_rows(const CdConvDesc* d, cudaStream_t st, int mode) {
   // convolutions of one micro-batch take 23.5 ms instead of 27.2 ms.
   const int tiles256 = p.tiles_x * cd_cdiv(d->Hg, kR256TH) * p.tiles_n * p.tiles_co;
   // The 16 x 16 kernel stages at most one epilogue operand per slice, so a launch with both resid and aux takes the 16 x 8 tiles.
+  // Its TMA output stores clip the channel dimension only in 16-byte units: with Cout % 4 != 0 they write zeros into the output
+  // row up to the next multiple of 4 channels (the Model's 3-channel conv_out, or the live columns of a neighbouring slice), so
+  // such a launch takes the 16 x 8 tiles, whose epilogue stores element by element.
   const bool rows256 = (mode == 4 || (by_shape && 4 * tiles256 >= 3 * sms)) && d->oys == 1 && d->oxs == 1 && d->oy0 == 0 &&
-                       d->ox0 == 0 && d->Ho == d->Hg && d->Wo == d->Wg && !(d->resid && d->act == CD_ACT_GELU_BWD);
+                       d->ox0 == 0 && d->Ho == d->Hg && d->Wo == d->Wg && !(d->resid && d->act == CD_ACT_GELU_BWD) &&
+                       d->Cout % 4 == 0;
   if (rows256) { p.TH = kR256TH; p.tiles_y = cd_cdiv(d->Hg, kR256TH); p.total_tiles = tiles256; }
   const CUtensorMapDataType dt = g_tf32_map_dtype ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUtensorMap maps[7] = {};

@@ -188,8 +188,11 @@ def _record_calls():
     try:
         yield calls
     finally:
-        for m in mods:
-            m.call = orig
+        # a package module first imported inside the context (model2_train, on the first training forward of a Model) took
+        # `call` from the patched _lib: give it the real one back too, or every later recording misses its calls
+        for m in list(sys.modules.values()):
+            if getattr(m, 'call', None) is rec:
+                m.call = orig
 
 
 def _parameter_gradient_calls(calls):
