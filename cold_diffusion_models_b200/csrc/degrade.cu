@@ -681,6 +681,102 @@ extern "C" int cd_noise_step(const float* img, const float* x1_bar, const float*
 }
 
 // -------------------------------------------------------------------------------------------------------------
+// Strided reverse steps (cd_noise_step_to, cd_fade_step_to): the update of cd_noise_step / cd_fade_step from level t to any
+// level s < t, x_s = img - D(x1, t) + D(x1, s), with D(x1, 0) = x1, in the same expressions as the one-step kernels.  s = t - 1
+// launches the one-step kernel itself: the compiler may contract the same expressions into different FMAs in another kernel,
+// and a K = T strided loop must be the one-step loop bit for bit.  kVec = 4: four consecutive elements per thread and
+// iteration, with 16-byte loads and stores (every operand 16-byte aligned; for the fade tables also HW % 4 == 0, so that the
+// four share one weight row); the n % 4 tail and misaligned operands take kVec = 1.
+// -------------------------------------------------------------------------------------------------------------
+namespace {
+__device__ __forceinline__ float noise_step_to_elem(float im, float xv, float nz, int mode, int s, float a1, float b1, float a2,
+                                                    float b2) {
+  const float x2 = mode == 0 ? (im - a1 * xv) / b1 : nz;
+  const float xt_bar = a1 * xv + b1 * x2;
+  const float xs = (s != 0) ? a2 * xv + b2 * x2 : xv;
+  return im - xt_bar + xs;
+}
+__device__ __forceinline__ float fade_step_to_elem(float im, float xv, float ev, float a1, float o1, bool to_clean, float a2, float o2) {
+  const float xt_bar = a1 * xv + o1 * ev;
+  float xs = xv;
+  if (!to_clean) xs = a2 * xv + o2 * ev;
+  return im - xt_bar + xs;
+}
+template <int kVec>
+__global__ void noise_step_to_kernel(const float* __restrict__ img, const float* __restrict__ x1, const float* __restrict__ noise,
+                                     int mode, int t, int s, const float* __restrict__ sa, const float* __restrict__ sb, long long n,
+                                     float* __restrict__ out) {
+  const float a1 = sa[t - 1], b1 = sb[t - 1];
+  const float a2 = s != 0 ? sa[s - 1] : 0.f, b2 = s != 0 ? sb[s - 1] : 0.f;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  long long i0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (kVec == 4) {
+    const long long n4 = n / 4;
+    for (long long i = i0; i < n4; i += stride) {
+      const float4 im = __ldg(reinterpret_cast<const float4*>(img) + i), xv = __ldg(reinterpret_cast<const float4*>(x1) + i);
+      const float4 nz = mode == 0 ? make_float4(0.f, 0.f, 0.f, 0.f) : __ldg(reinterpret_cast<const float4*>(noise) + i);
+      reinterpret_cast<float4*>(out)[i] = make_float4(noise_step_to_elem(im.x, xv.x, nz.x, mode, s, a1, b1, a2, b2),
+                                                      noise_step_to_elem(im.y, xv.y, nz.y, mode, s, a1, b1, a2, b2),
+                                                      noise_step_to_elem(im.z, xv.z, nz.z, mode, s, a1, b1, a2, b2),
+                                                      noise_step_to_elem(im.w, xv.w, nz.w, mode, s, a1, b1, a2, b2));
+    }
+    i0 += n4 * 4;
+  }
+  for (long long i = i0; i < n; i += stride)
+    out[i] = noise_step_to_elem(img[i], x1[i], mode == 0 ? 0.f : noise[i], mode, s, a1, b1, a2, b2);
+}
+template <int kVec>
+__global__ void fade_step_to_kernel(const float* __restrict__ img, const float* __restrict__ x1, const float* __restrict__ x2,
+                                    int t, int s, const float* __restrict__ al, const float* __restrict__ om, int HW, long long n,
+                                    float* __restrict__ out) {
+  const float* al1 = al + static_cast<long long>(t - 1) * HW;
+  const float* om1 = om + static_cast<long long>(t - 1) * HW;
+  const bool to_clean = s == 0;
+  const float* al2 = to_clean ? al1 : al + static_cast<long long>(s - 1) * HW;   // not read when s == 0
+  const float* om2 = to_clean ? om1 : om + static_cast<long long>(s - 1) * HW;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  long long i0 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (kVec == 4) {
+    const long long n4 = n / 4;
+    for (long long i = i0; i < n4; i += stride) {
+      const int p4 = static_cast<int>((i * 4) % HW) / 4;
+      const float4 im = __ldg(reinterpret_cast<const float4*>(img) + i), xv = __ldg(reinterpret_cast<const float4*>(x1) + i);
+      const float4 ev = __ldg(reinterpret_cast<const float4*>(x2) + i);
+      const float4 a1 = __ldg(reinterpret_cast<const float4*>(al1) + p4), o1 = __ldg(reinterpret_cast<const float4*>(om1) + p4);
+      float4 a2 = a1, o2 = o1;
+      if (!to_clean) { a2 = __ldg(reinterpret_cast<const float4*>(al2) + p4); o2 = __ldg(reinterpret_cast<const float4*>(om2) + p4); }
+      reinterpret_cast<float4*>(out)[i] = make_float4(fade_step_to_elem(im.x, xv.x, ev.x, a1.x, o1.x, to_clean, a2.x, o2.x),
+                                                      fade_step_to_elem(im.y, xv.y, ev.y, a1.y, o1.y, to_clean, a2.y, o2.y),
+                                                      fade_step_to_elem(im.z, xv.z, ev.z, a1.z, o1.z, to_clean, a2.z, o2.z),
+                                                      fade_step_to_elem(im.w, xv.w, ev.w, a1.w, o1.w, to_clean, a2.w, o2.w));
+    }
+    i0 += n4 * 4;
+  }
+  for (long long i = i0; i < n; i += stride) {
+    const int pix = static_cast<int>(i % HW);
+    out[i] = fade_step_to_elem(img[i], x1[i], x2[i], al1[pix], om1[pix], to_clean, to_clean ? 0.f : al2[pix],
+                               to_clean ? 0.f : om2[pix]);
+  }
+}
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+}  // namespace
+
+extern "C" int cd_noise_step_to(const float* img, const float* x1_bar, const float* noise, int mode, int t, int s,
+                                const float* sqrt_ac, const float* sqrt_1mac, int64_t n, float* out, void* stream) {
+  CD_REQUIRE(0 <= s && s < t && (mode == 0 || (mode == 1 && noise)) && n >= 0, "cd_noise_step_to: bad arguments");
+  if (n == 0) return 0;
+  if (s == t - 1) return cd_noise_step(img, x1_bar, noise, mode, t, sqrt_ac, sqrt_1mac, n, out, stream);
+  const bool vec = aligned16(img) && aligned16(x1_bar) && aligned16(out) && (mode == 0 || aligned16(noise));
+  int blocks = cd_cdiv(vec ? n / 4 : n, 256); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
+  if (vec)
+    noise_step_to_kernel<4><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(img, x1_bar, noise, mode, t, s, sqrt_ac, sqrt_1mac, n, out);
+  else
+    noise_step_to_kernel<1><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(img, x1_bar, noise, mode, t, s, sqrt_ac, sqrt_1mac, n, out);
+  CD_LAUNCH_CHECK();
+  return 0;
+}
+
+// -------------------------------------------------------------------------------------------------------------
 // Fade-to-colour generation (defading-generation-diffusion-pytorch/defading_diffusion_pytorch/defading_diffusion_pytorch.py,
 // "DFGEN"): the schedule is a per-PIXEL weight, alphas[t][y][x] = cumulative product of the fade kernels (DFGEN:320-344),
 // q_sample = alphas[t_b] * x1 + one_minus_alphas[t_b] * x2 (DFGEN:543-548), reverse step = img - xt_bar + xt_sub1_bar with
@@ -760,6 +856,23 @@ extern "C" int cd_fade_step(const float* img, const float* x1_bar, const float* 
   const long long n = static_cast<long long>(B) * C * HW;
   int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
   fade_step_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(img, x1_bar, x2, t, alphas, one_minus_alphas, HW, n, out);
+  CD_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int cd_fade_step_to(const float* img, const float* x1_bar, const float* x2, int t, int s, const float* alphas,
+                               const float* one_minus_alphas, int B, int C, int HW, float* out, void* stream) {
+  CD_REQUIRE(0 <= s && s < t && x2 && B >= 0 && C >= 1 && HW >= 1, "cd_fade_step_to: bad arguments");
+  const long long n = static_cast<long long>(B) * C * HW;
+  if (n == 0) return 0;
+  if (s == t - 1) return cd_fade_step(img, x1_bar, x2, t, alphas, one_minus_alphas, B, C, HW, out, stream);
+  const bool vec = HW % 4 == 0 && aligned16(img) && aligned16(x1_bar) && aligned16(x2) && aligned16(out) && aligned16(alphas) &&
+                   aligned16(one_minus_alphas);
+  int blocks = cd_cdiv(vec ? n / 4 : n, 256); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
+  if (vec)
+    fade_step_to_kernel<4><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(img, x1_bar, x2, t, s, alphas, one_minus_alphas, HW, n, out);
+  else
+    fade_step_to_kernel<1><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(img, x1_bar, x2, t, s, alphas, one_minus_alphas, HW, n, out);
   CD_LAUNCH_CHECK();
   return 0;
 }

@@ -14,6 +14,7 @@ import torch.nn.functional as F  # noqa: F401  (kept for API familiarity; not us
 from ._lib import call, ptr, stream
 from .autograd import BlurDegrade, refuse_grad
 from .degradation import build_blur_operators
+from .strided import refuse_strided, reverse_levels
 
 
 class _LossFn(torch.autograd.Function):
@@ -142,31 +143,52 @@ class GaussianDiffusion(nn.Module):
         return self.p_losses(x, t, *args, **kwargs)
 
     # ---- reverse process -----------------------------------------------------------------------------
-    def _reverse_step(self, img, x0_hat, t):
-        """one step of Algorithm 1 ('default') or Algorithm 2 ('x0_step_down') (DB:428-451)."""
+    def _reverse_step(self, img, x0_hat, t, lo=None):
+        """one step of Algorithm 1 ('default') or Algorithm 2 ('x0_step_down') (DB:428-451) from level t to level lo
+        (t - 1 unless given: the strided loop of `sample(steps=...)`)"""
         T = self.num_timesteps
+        if lo is None:
+            lo = t - 1
         if self.sampling_routine == 'default':
             if self.blur_routine == 'Individual_Incremental':
-                return self._apply_op(x0_hat, (t - 2) % T, single=True)
-            return self._apply_op(x0_hat, t - 2)
+                return self._apply_op(x0_hat, (lo - 1) % T, single=True)
+            return self._apply_op(x0_hat, lo - 1)
         elif self.sampling_routine == 'x0_step_down':
-            return self._step_down(img, x0_hat, t)
+            return self._step_down(img, x0_hat, t, lo)
         return x0_hat          # unknown routine: the reference leaves x = x0_hat
 
-    def _step_down(self, img, x0_hat, t):
-        """Algorithm 2: x_{t-1} = x_t - D(x0_hat, t) + D(x0_hat, t-1) with the cumulative operators (DB:436-451)."""
+    def _step_down(self, img, x0_hat, t, lo=None):
+        """Algorithm 2: x_{lo} = x_t - D(x0_hat, t) + D(x0_hat, lo) with the cumulative operators, lo = t-1 unless given
+        (DB:436-451)"""
+        if lo is None:
+            lo = t - 1
         out = torch.empty_like(img)
         B, Cc, H, W = img.shape
         call('cd_blur_step_down', ptr(img.contiguous()), ptr(x0_hat.contiguous()), ptr(out), ptr(self._ops_cum),
-             t - 1, t - 2, B, Cc, H, self.num_timesteps, int(self.discrete), stream())
+             t - 1, lo - 1, B, Cc, H, self.num_timesteps, int(self.discrete), stream())
         return out
 
+    def _check_strided(self, steps):
+        """the routines whose one-step update has no strided counterpart (ValueError when steps is given): train routines other
+        than 'Final' (the network output is the next image), unknown sampling routines (x = x0_hat), and 'default' with
+        'Individual_Incremental' blur, whose update applies the single kernel K_{t-2} (K_{T-1} at the last step) rather
+        than D(x0_hat, t-1).  Its 'x0_step_down' forms D(x0_hat, s) from the cumulative operators, as q_sample does."""
+        if self.train_routine != 'Final':
+            refuse_strided(steps, 'deblurring', "train_routine=%r" % self.train_routine)
+        if self.sampling_routine not in ('default', 'x0_step_down'):
+            refuse_strided(steps, 'deblurring', "sampling_routine=%r" % self.sampling_routine)
+        if self.sampling_routine == 'default' and self.blur_routine == 'Individual_Incremental':
+            refuse_strided(steps, 'deblurring', "sampling_routine='default' with blur_routine='Individual_Incremental'")
+
     @torch.no_grad()
-    def sample(self, batch_size=16, img=None, t=None, _noise=None):
-        """DB:393-455 -> (xt, direct_recons, img)"""
-        self.denoise_fn.eval()
+    def sample(self, batch_size=16, img=None, t=None, _noise=None, *, steps=None):
+        """DB:393-455 -> (xt, direct_recons, img).  steps=K: K reverse steps through the levels of strided.reverse_levels
+        instead of all t (None: every level, the reference's loop)"""
         if t is None:
             t = self.num_timesteps
+        self._check_strided(steps)
+        levels = reverse_levels(t, steps)
+        self.denoise_fn.eval()
         img = self._degrade_to(img, t)
         if self.discrete:
             img = torch.mean(img, [2, 3], keepdim=True).expand_as(img).contiguous()
@@ -174,15 +196,14 @@ class GaussianDiffusion(nn.Module):
             img = img + _noise
         xt = img
         direct_recons = None
-        while t:
-            step = torch.full((batch_size,), t - 1, dtype=torch.long, device=img.device)
+        for hi, lo in zip(levels, levels[1:]):
+            step = torch.full((batch_size,), hi - 1, dtype=torch.long, device=img.device)
             x = self.denoise_fn(img, step)
             if self.train_routine == 'Final':
                 if direct_recons is None:
                     direct_recons = x
-                x = self._reverse_step(img, x, t)
+                x = self._reverse_step(img, x, hi, lo)
             img = x
-            t = t - 1
         self.denoise_fn.train()
         return xt, direct_recons, img
 

@@ -13,6 +13,7 @@ from ._lib import call, ptr, stream
 from .autograd import MaskDegrade, refuse_grad
 from .deblurring import _LossFn
 from .degradation import gaussian_taps
+from .strided import refuse_strided, reverse_levels
 
 
 class GaussianDiffusion(nn.Module):
@@ -106,32 +107,36 @@ class GaussianDiffusion(nn.Module):
         return self.p_losses(x, t, *args, **kwargs)
 
     @torch.no_grad()
-    def sample(self, batch_size=16, faded_recon_sample=None, t=None, _offsets=None):
-        """DFG:355-424 -> (xt, direct_recons, recon_sample)"""
-        x = faded_recon_sample
-        rx, ry = _offsets if _offsets is not None else self._offsets(batch_size, x.device)
+    def sample(self, batch_size=16, faded_recon_sample=None, t=None, _offsets=None, *, steps=None):
+        """DFG:355-424 -> (xt, direct_recons, recon_sample).  steps=K: K reverse steps through the levels of
+        strided.reverse_levels instead of all t (None: every level, the reference's loop); the 'Random_*' routines keep one
+        window per sample for the whole loop.  Unknown sampling routines (which leave x as it is) raise ValueError with it."""
+        if self.sampling_routine not in ('default', 'x0_step_down'):
+            refuse_strided(steps, 'defading', "sampling_routine=%r" % self.sampling_routine)
         if t is None:
             t = self.num_timesteps
+        levels = reverse_levels(t, steps)
+        x = faded_recon_sample
+        rx, ry = _offsets if _offsets is not None else self._offsets(batch_size, x.device)
         x = self._fade(x, t - 1, rx, ry, quantize=self.discrete)
         xt = x
         direct_recons = None
         recon = None
         B, Cc, S, _ = x.shape
         MS = self._masks_cum.shape[-1]
-        while t:
-            step = torch.full((batch_size,), t - 1, dtype=torch.long, device=x.device)
+        for hi, lo in zip(levels, levels[1:]):
+            step = torch.full((batch_size,), hi - 1, dtype=torch.long, device=x.device)
             recon = self.defade_fn(x, step)
             if direct_recons is None:
                 direct_recons = recon
             if self.sampling_routine == 'default':
-                x = self._fade(recon, t - 2, rx, ry)
+                x = self._fade(recon, lo - 1, rx, ry)
             elif self.sampling_routine == 'x0_step_down':
                 out = torch.empty_like(x)
                 call('cd_mask_step_down', ptr(x.contiguous()), ptr(recon.contiguous()), ptr(out), ptr(self._masks_cum),
-                     t - 1, t - 2, ptr(rx), ptr(ry), B, Cc, S, MS, stream())
+                     hi - 1, lo - 1, ptr(rx), ptr(ry), B, Cc, S, MS, stream())
                 x = out
             recon = x
-            t -= 1
         return xt, direct_recons, recon
 
     @torch.no_grad()

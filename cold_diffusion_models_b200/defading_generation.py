@@ -5,7 +5,8 @@ The image fades towards a second image x2 (the driver uses a constant random col
 weight: alphas[t] = prod_{i<=t} K_i of the Gaussian fade kernels (DFGEN:313-344), q_sample = alphas[t_b] x1 +
 (1 - alphas[t_b]) x2 (DFGEN:543-548).  The reference gathers the (1,S,S) weight planes with a Python loop over the
 batch (`extract`, DFGEN:285-294); here q_sample and the Algorithm-2 update are one elementwise kernel each
-(cd_fade_lerp / cd_fade_step) indexing the resident [T][S][S] tables per sample."""
+(cd_fade_lerp / cd_fade_step) indexing the resident [T][S][S] tables per sample; `sample(steps=K)` strides with
+cd_fade_step_to."""
 import ctypes as C  # noqa: F401
 import torch
 from torch import nn
@@ -14,6 +15,7 @@ from ._lib import call, ptr, stream
 from .autograd import LerpDegrade
 from .deblurring import _LossFn
 from .degradation import gaussian_taps
+from .strided import reverse_levels
 
 
 def get_fade_kernel(dims, std):
@@ -141,14 +143,35 @@ class GaussianDiffusion(nn.Module):
             t = t - 1
         return direct_recons, img
 
+    def _reverse_strided(self, batch_size, img, x2, levels):
+        """_reverse through the given levels (strided.reverse_levels): img <- img - D(x1_bar, hi) + D(x1_bar, lo) in one
+        cd_fade_step_to per pair"""
+        B, Cc, H, W = img.shape
+        direct_recons = None
+        for hi, lo in zip(levels, levels[1:]):
+            step = torch.full((batch_size,), hi - 1, dtype=torch.long, device=img.device)
+            x1_bar = self.denoise_fn(img, step)
+            if direct_recons is None:
+                direct_recons = x1_bar
+            out = torch.empty_like(img)
+            call('cd_fade_step_to', ptr(img), ptr(x1_bar.contiguous()), ptr(x2), hi, lo, ptr(self.alphas), ptr(self.one_minus_alphas),
+                 B, Cc, H * W, ptr(out), stream())
+            img = out
+        return direct_recons, img
+
     @torch.no_grad()
-    def sample(self, batch_size=16, img=None, t=None):
-        """DFGEN:385-418 -> (xt, direct_recons, img)"""
-        self.denoise_fn.eval()
+    def sample(self, batch_size=16, img=None, t=None, *, steps=None):
+        """DFGEN:385-418 -> (xt, direct_recons, img).  steps=K: K reverse steps through the levels of strided.reverse_levels
+        (cd_fade_step_to) instead of all t (None: every level, the reference's loop)"""
         if t is None:
             t = self.num_timesteps
+        levels = None if steps is None else reverse_levels(t, steps)
+        self.denoise_fn.eval()
         orig = img.contiguous().float()
-        direct_recons, out = self._reverse(batch_size, orig, orig, t)
+        if levels is None:
+            direct_recons, out = self._reverse(batch_size, orig, orig, t)
+        else:
+            direct_recons, out = self._reverse_strided(batch_size, orig, orig, levels)
         self.denoise_fn.train()
         return orig, direct_recons, out
 

@@ -11,6 +11,7 @@ from torch import nn
 from ._lib import call, ptr, stream
 from .autograd import LerpDegrade
 from .deblurring import _LossFn
+from .strided import reverse_levels
 
 
 def cosine_beta_schedule(timesteps, s=0.008):
@@ -91,6 +92,13 @@ class GaussianDiffusion(nn.Module):
              ptr(self.sqrt_alphas_cumprod), ptr(self.sqrt_one_minus_alphas_cumprod), C.c_int64(img.numel()), ptr(out), stream())
         return out
 
+    def _step_to(self, img, x1_bar, noise, mode, t, s):
+        """the reverse step from level t to any level s < t (cd_noise_step_to; s = t - 1 is _step's result bit for bit)"""
+        out = torch.empty_like(img)
+        call('cd_noise_step_to', ptr(img.contiguous()), ptr(x1_bar.contiguous()), ptr(noise), mode, t, s,
+             ptr(self.sqrt_alphas_cumprod), ptr(self.sqrt_one_minus_alphas_cumprod), C.c_int64(img.numel()), ptr(out), stream())
+        return out
+
     def _reverse(self, batch_size, img, t, mode, noise, collect=None):
         direct_recons = None
         while t:
@@ -104,14 +112,30 @@ class GaussianDiffusion(nn.Module):
             t = t - 1
         return direct_recons, img
 
+    def _reverse_strided(self, batch_size, img, levels, mode, noise):
+        """_reverse through the given levels (strided.reverse_levels), one cd_noise_step_to per pair"""
+        direct_recons = None
+        for hi, lo in zip(levels, levels[1:]):
+            step = torch.full((batch_size,), hi - 1, dtype=torch.long, device=img.device)
+            x1_bar = self.denoise_fn(img, step)
+            if direct_recons is None:
+                direct_recons = x1_bar
+            img = self._step_to(img, x1_bar, noise, mode, hi, lo)
+        return direct_recons, img
+
     @torch.no_grad()
-    def sample(self, batch_size=16, img=None, t=None):
-        """DN:342-375 (always the 'ddim'-style estimate of x2) -> (xt, direct_recons, img)"""
-        self.denoise_fn.eval()
+    def sample(self, batch_size=16, img=None, t=None, *, steps=None):
+        """DN:342-375 (always the 'ddim'-style estimate of x2) -> (xt, direct_recons, img).  steps=K: K reverse steps through
+        the levels of strided.reverse_levels (cd_noise_step_to) instead of all t (None: every level, the reference's loop)"""
         if t is None:
             t = self.num_timesteps
+        levels = None if steps is None else reverse_levels(t, steps)
+        self.denoise_fn.eval()
         xt = img
-        direct_recons, img = self._reverse(batch_size, img.contiguous().float(), t, 0, None)
+        if levels is None:
+            direct_recons, img = self._reverse(batch_size, img.contiguous().float(), t, 0, None)
+        else:
+            direct_recons, img = self._reverse_strided(batch_size, img.contiguous().float(), levels, 0, None)
         self.denoise_fn.train()
         return xt, direct_recons, img
 

@@ -18,6 +18,7 @@ from ._lib import call, ptr, stream
 from .autograd import BlurDegrade
 from .deblurring import _LossFn
 from .degradation import gaussian_taps, blur_matrix
+from .strided import refuse_strided, reverse_levels
 
 
 def step_specs(resolution_routine, timesteps, image_size):
@@ -199,34 +200,43 @@ class GaussianDiffusion(nn.Module):
         return self.p_losses(x, t, *args, **kwargs)
 
     # ---- reverse process -----------------------------------------------------------------------------------
-    def _reverse_step(self, img, x0_hat, t):
+    def _reverse_step(self, img, x0_hat, t, lo=None):
+        """Algorithm 1 / 2 from level t to level lo (t - 1 unless given) with the tabulated cumulative operators"""
+        if lo is None:
+            lo = t - 1
         if self.sampling_routine == 'default':
-            return self._apply_op(x0_hat, t - 2)
+            return self._apply_op(x0_hat, lo - 1)
         elif self.sampling_routine == 'x0_step_down':
             out = torch.empty_like(img)
             B, Cc, H, W = img.shape
             call('cd_blur_step_down', ptr(img.contiguous()), ptr(x0_hat.contiguous()), ptr(out), ptr(self._ops_cum),
-                 t - 1, t - 2, B, Cc, H, self.num_timesteps, 0, stream())
+                 t - 1, lo - 1, B, Cc, H, self.num_timesteps, 0, stream())
             return out
         return x0_hat
 
     @torch.no_grad()
-    def sample(self, batch_size=16, img=None, t=None):
-        """RS:417-459 -> (xt, direct_recons, img)"""
+    def sample(self, batch_size=16, img=None, t=None, *, steps=None):
+        """RS:417-459 -> (xt, direct_recons, img).  steps=K: K reverse steps through the levels of strided.reverse_levels
+        instead of all t (None: every level, the reference's loop).  Train routines other than 'Final' (the network output is
+        the next image) and unknown sampling routines have no strided form: ValueError."""
+        if self.train_routine != 'Final':
+            refuse_strided(steps, 'resolution', "train_routine=%r" % self.train_routine)
+        if self.sampling_routine not in ('default', 'x0_step_down'):
+            refuse_strided(steps, 'resolution', "sampling_routine=%r" % self.sampling_routine)
         if t is None:
             t = self.num_timesteps
+        levels = reverse_levels(t, steps)
         img = self._apply_op(img, t - 1)
         xt = img
         direct_recons = None
-        while t:
-            step = torch.full((batch_size,), t - 1, dtype=torch.long, device=img.device)
+        for hi, lo in zip(levels, levels[1:]):
+            step = torch.full((batch_size,), hi - 1, dtype=torch.long, device=img.device)
             x = self.denoise_fn(img, step)
             if self.train_routine == 'Final':
                 if direct_recons is None:
                     direct_recons = x
-                x = self._reverse_step(img, x, t)
+                x = self._reverse_step(img, x, hi, lo)
             img = x
-            t = t - 1
         return xt, direct_recons, img
 
     @torch.no_grad()

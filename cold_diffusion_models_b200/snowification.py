@@ -27,6 +27,7 @@ from ._lib import call, ptr, stream
 from .autograd import ChanmixDegrade, refuse_grad
 from .deblurring import _LossFn
 from .degradation import gaussian_taps
+from .strided import refuse_strided, reverse_levels
 from .train_graph import recording
 
 
@@ -363,14 +364,21 @@ class GaussianDiffusion(nn.Module):
         return self.p_losses(x, t, None, *args, **kwargs)      # the reference's t_pred is drawn but never used (SN:440-447)
 
     # ---- reverse process --------------------------------------------------------------------------------------------
+    _FINAL_ROUTINES = ('Final', 'Final_random_mean', 'Final_small_noise', 'Final_random_mean_and_actual')
+
     @torch.no_grad()
-    def sample_one_step(self, img, t, init_pred=None):
-        """SN:195-245 -> (x, direct_recons); t is a per-sample int64 tensor."""
+    def sample_one_step(self, img, t, init_pred=None, _t_lo=None):
+        """SN:195-245 -> (x, direct_recons); t is a per-sample int64 tensor.  _t_lo (the strided loop of `sample(steps=...)`):
+        the network time of the level to step down to, per sample, in place of t - 1; the update then indexes D with
+        _t_lo - 1 where the one-step update indexes it with t - 2 (the reference's offsets)."""
         x = self.prediction_step_t(img, t, init_pred)
         direct_recons = x.clone()
-        if self.train_routine in ['Final', 'Final_random_mean', 'Final_small_noise', 'Final_random_mean_and_actual']:
+        if self.train_routine in self._FINAL_ROUTINES:
             if self.sampling_routine == 'default':
-                x = self._degrade(x, t, -2)                                        # t_b - 1 steps per row
+                if _t_lo is not None:
+                    x = self._degrade(x, _t_lo, -1)
+                else:
+                    x = self._degrade(x, t, -2)                                    # t_b - 1 steps per row
             elif self.sampling_routine == 'x0_step_down':
                 src = x
                 if self.recon_noise_std > 0.0 and isinstance(self.forward_process, DeColorization):
@@ -378,7 +386,7 @@ class GaussianDiffusion(nn.Module):
                     src = x + torch.normal(0.0, self.recon_noise_std, size=x.size(), device=x.device)
                 # x_times_sub_1 is re-cloned from ALL rows each iteration (SN:229-233): rows that finished before the
                 # last iteration end with x_times_sub_1 == x_times, i.e. the update leaves them at `img`.
-                t_lo = torch.where(t == torch.max(t), t - 1, t)
+                t_lo = torch.where(t == torch.max(t), t - 1, t) if _t_lo is None else _t_lo
                 x = self._degrade(src, t, -1, xt=img, t_lo=t_lo, lo_off=-1)
         elif self.train_routine == 'Step':
             pass
@@ -399,23 +407,31 @@ class GaussianDiffusion(nn.Module):
         return img_new
 
     @torch.no_grad()
-    def sample(self, batch_size=16, img=None, t=None):
-        """SN:259-295 -> {'xt', 'direct_recons', 'recon'}"""
-        self.forward_process.reset_parameters(batch_size=batch_size)
+    def sample(self, batch_size=16, img=None, t=None, *, steps=None):
+        """SN:259-295 -> {'xt', 'direct_recons', 'recon'}.  steps=K: K reverse steps through the levels of
+        strided.reverse_levels instead of all t (None: every level, the reference's loop), with the one-step update's index
+        offsets and per-sample snow layers.  The 'Step' / 'Step_Gradient' train routines (the network output is the next image
+        or the step to it) and unknown sampling routines have no strided form: ValueError."""
+        if self.train_routine not in self._FINAL_ROUTINES:
+            refuse_strided(steps, 'snowification', "train_routine=%r" % self.train_routine)
+        if self.sampling_routine not in ('default', 'x0_step_down'):
+            refuse_strided(steps, 'snowification', "sampling_routine=%r" % self.sampling_routine)
         if t is None:
             t = self.num_timesteps
+        levels = reverse_levels(t, steps)
+        self.forward_process.reset_parameters(batch_size=batch_size)
         og_img = img
         tt = torch.full((img.shape[0],), t, dtype=torch.long, device=img.device)
         img = self._degrade(og_img, tt, -1)
         xt = img
         direct_recons = None
-        while t:
-            step = torch.full((batch_size,), t - 1, dtype=torch.long, device=img.device)
-            x, cur = self.sample_one_step(img, step)
+        for hi, lo in zip(levels, levels[1:]):
+            step = torch.full((batch_size,), hi - 1, dtype=torch.long, device=img.device)
+            t_lo = None if steps is None else torch.full((batch_size,), lo - 1, dtype=torch.long, device=img.device)
+            x, cur = self.sample_one_step(img, step, _t_lo=t_lo)
             if direct_recons is None:
                 direct_recons = cur
             img = x
-            t = t - 1
         if self.to_lab:                                                             # SN:287-290
             xt, direct_recons, img = lab2rgb(xt), lab2rgb(direct_recons), lab2rgb(img)
         return {'xt': xt, 'direct_recons': direct_recons, 'recon': img}

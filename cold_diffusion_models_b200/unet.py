@@ -158,6 +158,10 @@ class Unet(nn.Module):
         return new
 
     def _apply(self, fn, *a, **k):
+        if getattr(self, '_engine', None) is not None:
+            # free the captured graphs now: the engine sits in a reference cycle, and a graph that the garbage collector
+            # destroys while another graph is being captured invalidates that capture
+            self._engine.drop_graphs()
         self._engine = None                     # parameters moved/cast: rebuild packed weights and graphs lazily
         return super()._apply(fn, *a, **k)
 

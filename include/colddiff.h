@@ -294,6 +294,11 @@ int cd_noise_lerp(const float* x1, const float* x2, const int64_t* t, int t_scal
                   const float* sqrt_1mac, int64_t per_sample, int64_t n, float* out, void* stream);
 int cd_noise_step(const float* img, const float* x1_bar, const float* noise, int mode, int t, const float* sqrt_ac,
                   const float* sqrt_1mac, int64_t n, float* out, void* stream);
+/* cd_noise_step_to: the same reverse step from level t to any level s, 0 <= s < t (strided sampling, `sample(steps=K)`):
+ * img - xt_bar + xs_bar with xt_bar from sqrt_ac / sqrt_1mac at t-1 and xs_bar at s-1; s = 0: xs_bar = x1_bar (the clean
+ * estimate).  Both modes of cd_noise_step; s = t-1 runs cd_noise_step itself (its bits).                              */
+int cd_noise_step_to(const float* img, const float* x1_bar, const float* noise, int mode, int t, int s, const float* sqrt_ac,
+                     const float* sqrt_1mac, int64_t n, float* out, void* stream);
 /* Fade-to-colour generation (defading-generation-diffusion-pytorch/defading_diffusion_pytorch/defading_diffusion_pytorch.py,
  * "DFGEN"): per-pixel schedule alphas / one_minus_alphas [T][HW] (DFGEN:320-344, 371-381).
  *   cd_fade_lerp : q_sample = alphas[t_b] * x1 + one_minus_alphas[t_b] * x2 (t: int64 [B], or NULL -> t_scalar)  (DFGEN:543-548)
@@ -302,6 +307,10 @@ int cd_fade_lerp(const float* x1, const float* x2, const int64_t* t, int t_scala
                  const float* one_minus_alphas, int B, int C, int HW, float* out, void* stream);
 int cd_fade_step(const float* img, const float* x1_bar, const float* x2, int t, const float* alphas,
                  const float* one_minus_alphas, int B, int C, int HW, float* out, void* stream);
+/* cd_fade_step_to: cd_fade_step from level t to any level s, 0 <= s < t: the tables are read at rows t-1 and s-1; s = 0 goes
+ * to the clean estimate x1_bar.  s = t-1 runs cd_fade_step itself (its bits).                                             */
+int cd_fade_step_to(const float* img, const float* x1_bar, const float* x2, int t, int s, const float* alphas,
+                    const float* one_minus_alphas, int B, int C, int HW, float* out, void* stream);
 /* cd_lerp2_adjoint: the gradients of out = wa[w] x1 + wb[w] x2 (cd_noise_lerp, cd_fade_lerp) from one pass over g [B][C][HW]:
  * ga = wa[w] g, gb = wb[w] g, with w = t_b (per_pixel = 0: per-sample scalars, cd_noise_lerp) or t_b * HW + pixel (per_pixel = 1:
  * [T][HW] tables, cd_fade_lerp).  t: int64 [B], or NULL -> t_scalar.  ga or gb may be NULL (that gradient is not written). */
