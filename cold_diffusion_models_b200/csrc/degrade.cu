@@ -91,10 +91,15 @@ __device__ __forceinline__ void plane_apply(const float* As, const float* Xs, fl
 // read only in step 1, Zs written in step 2 -> Zs = Xs)
 // kAdj: the adjoint A^T G A of the same operator (the gradient of A X A^T): A_idx is loaded transposed into As, and the
 // collapse at T-1 comes first -- the adjoint of X -> mean(A X A^T) 11^T is G -> A^T (mean(G) 11^T) A.
-template <bool kAdj>
+// kEpi (guided restoration; collapse_last and quantize are then 0): kEpiNone = the plain product; kEpiAxpy = A X A^T - w g
+// (the guided `default` update, and with w = 1, g = y the residual of the two-pass guidance gradient); kEpiGuide = the guidance
+// gradient A^T (A X A^T - g) A in one pass: the residual stays in shared memory and A is reloaded transposed over the used As.
+constexpr int kEpiNone = 0, kEpiAxpy = 1, kEpiGuide = 2;
+template <bool kAdj, int kEpi = kEpiNone>
 __global__ void __launch_bounds__(256)
 blur_apply_kernel(const float* __restrict__ x, float* __restrict__ out, const float* __restrict__ ops,
-                  const long long* __restrict__ t, int t_scalar, int S, int T, int collapse_last, int quantize) {
+                  const long long* __restrict__ t, int t_scalar, int S, int T, int collapse_last, int quantize,
+                  const float* __restrict__ g, float w) {
   extern __shared__ __align__(16) float sm[];
   const int ldp = S + 4;
   float* As = sm; float* Xs = As + S * S; float* Yt = Xs + S * ldp; float* scratch = Yt + S * ldp;
@@ -126,9 +131,25 @@ blur_apply_kernel(const float* __restrict__ x, float* __restrict__ out, const fl
     mean = block_sum(s, scratch) / (S * S);
   }
   const int per_row = S >> 2;
+  if constexpr (kEpi == kEpiGuide) {
+    // each thread rewrites the float4 slots it stores below; plane_apply ended with a barrier, so As is free
+    for (int i = threadIdx.x; i < (S * S) >> 2; i += blockDim.x) {
+      const int r = i / per_row, c = (i % per_row) * 4;
+      float4* z = reinterpret_cast<float4*>(Xs + r * ldp + c);
+      const float4 yv = __ldg(reinterpret_cast<const float4*>(g + pl * S * S) + i);
+      *z = make_float4(z->x - yv.x, z->y - yv.y, z->z - yv.z, z->w - yv.w);
+    }
+    if (idx >= 0) load_plane_transposed(As, ops + static_cast<long long>(idx) * S * S, S);
+    __syncthreads();
+    if (idx >= 0) plane_apply(As, Xs, Yt, Xs, S, ldp);
+  }
   for (int i = threadIdx.x; i < (S * S) >> 2; i += blockDim.x) {
     const int r = i / per_row, c = (i % per_row) * 4;
     float4 v = *reinterpret_cast<const float4*>(Xs + r * ldp + c);
+    if constexpr (kEpi == kEpiAxpy) {
+      const float4 gv = __ldg(reinterpret_cast<const float4*>(g + pl * S * S) + i);
+      v = make_float4(v.x - w * gv.x, v.y - w * gv.y, v.z - w * gv.z, v.w - w * gv.w);
+    }
     if (!kAdj && collapse) v = make_float4(mean, mean, mean, mean);
     if (quantize) {
       float* f = reinterpret_cast<float*>(&v);
@@ -146,9 +167,12 @@ blur_apply_kernel(const float* __restrict__ x, float* __restrict__ out, const fl
 
 // out = xt - A_hi xhat A_hi^T + A_lo xhat A_lo^T   (index -1 = identity).
 // smem: As | Xs | Yt (Z overwrites Xs; xhat is re-read from L2 for the second term) = 196 KB at S = 128.
+// kAxpy: the guided update, out - w g in the epilogue.
+template <bool kAxpy = false>
 __global__ void __launch_bounds__(256)
 blur_step_down_kernel(const float* __restrict__ xt, const float* __restrict__ xhat, float* __restrict__ out,
-                      const float* __restrict__ ops, int t_hi, int t_lo, int S, int T, int collapse_last) {
+                      const float* __restrict__ ops, int t_hi, int t_lo, int S, int T, int collapse_last,
+                      const float* __restrict__ g, float w) {
   extern __shared__ __align__(16) float sm[];
   const int ldp = S + 4;
   float* As = sm; float* Xs = As + S * S; float* Yt = Xs + S * ldp; float* scratch = Yt + S * ldp;
@@ -189,6 +213,10 @@ blur_step_down_kernel(const float* __restrict__ xt, const float* __restrict__ xh
     const float4 z = *reinterpret_cast<const float4*>(Xs + r * ldp + c);
     float4 o = d[nslot];
     o.x += z.x; o.y += z.y; o.z += z.z; o.w += z.w;
+    if constexpr (kAxpy) {
+      const float4 gv = __ldg(reinterpret_cast<const float4*>(g + pl * S * S) + i);
+      o = make_float4(o.x - w * gv.x, o.y - w * gv.y, o.z - w * gv.z, o.w - w * gv.w);
+    }
     reinterpret_cast<float4*>(out + pl * S * S)[i] = o;
   }
 }
@@ -414,11 +442,13 @@ __device__ __forceinline__ void strip_degrade(const float* __restrict__ ops, con
   strip_product<NQ, kAdj>(A, X, S, r0, sm, acc);
 }
 
-// kAdj: the adjoint A^T G A of the same operator (cd_blur_apply_adjoint; quantize is then 0)
-template <int NQ, bool kAdj>
+// kAdj: the adjoint A^T G A of the same operator (cd_blur_apply_adjoint; quantize is then 0).  kAxpy: out = D x - w g (the
+// guided `default` update, and the residual D x - y of the two-pass guidance gradient; quantize is then 0).
+template <int NQ, bool kAdj, bool kAxpy = false>
 __global__ void __launch_bounds__(kStripThreads, 1)
 blur_apply_strip_kernel(const float* __restrict__ x, float* __restrict__ out, const float* __restrict__ ops,
-                        const long long* __restrict__ t, int t_scalar, int C, int S, int T, int collapse_last, int quantize) {
+                        const long long* __restrict__ t, int t_scalar, int C, int S, int T, int collapse_last, int quantize,
+                        const float* __restrict__ g, float w) {
   extern __shared__ __align__(16) float sm[];
   const int nstrip = strip_cdiv(S, kStripR);
   const int pl = blockIdx.x / nstrip;                     // b * C + c; the strips of one plane are adjacent
@@ -439,15 +469,19 @@ blur_apply_strip_kernel(const float* __restrict__ x, float* __restrict__ out, co
         f[k] = qv * 2.f - 1.f;
       }
     }
+    if constexpr (kAxpy) {
+      const float4 gv = __ldg(reinterpret_cast<const float4*>(g + static_cast<long long>(pl) * S * S + o));
+      f[0] = f[0] - w * gv.x; f[1] = f[1] - w * gv.y; f[2] = f[2] - w * gv.z; f[3] = f[3] - w * gv.w;
+    }
     *reinterpret_cast<float4*>(op + o) = make_float4(f[0], f[1], f[2], f[3]);
   });
 }
 
-// out = xt - Z_hi + Z_lo: xt - Z_hi is parked in `out` and read back by the thread that wrote it
-template <int NQ>
+// out = xt - Z_hi + Z_lo: xt - Z_hi is parked in `out` and read back by the thread that wrote it.  kAxpy: minus w g as well.
+template <int NQ, bool kAxpy = false>
 __global__ void __launch_bounds__(kStripThreads, 1)
 blur_step_down_strip_kernel(const float* __restrict__ xt, const float* __restrict__ xhat, float* out, const float* __restrict__ ops,
-                            int t_hi, int t_lo, int S, int T, int collapse_last) {
+                            int t_hi, int t_lo, int S, int T, int collapse_last, const float* __restrict__ g, float w) {
   extern __shared__ __align__(16) float sm[];
   const int nstrip = strip_cdiv(S, kStripR);
   const int pl = blockIdx.x / nstrip;
@@ -466,6 +500,10 @@ blur_step_down_strip_kernel(const float* __restrict__ xt, const float* __restric
   strip_for_each<NQ>(S, r0, [&](int q, int a, long long o) {
     float4 d = *reinterpret_cast<const float4*>(op + o);
     d.x += acc[q][a][0]; d.y += acc[q][a][1]; d.z += acc[q][a][2]; d.w += acc[q][a][3];
+    if constexpr (kAxpy) {
+      const float4 gv = __ldg(reinterpret_cast<const float4*>(g + static_cast<long long>(pl) * S * S + o));
+      d = make_float4(d.x - w * gv.x, d.y - w * gv.y, d.z - w * gv.z, d.w - w * gv.w);
+    }
     *reinterpret_cast<float4*>(op + o) = d;
   });
 }
@@ -530,49 +568,55 @@ static int strip_grid(int B, int C, int S, unsigned* grid) {
   return 0;
 }
 
-template <int NQ, bool kAdj>
+template <int NQ, bool kAdj, bool kAxpy = false>
 static int blur_apply_strips(const float* x, float* out, const float* ops, const int64_t* t, int t_scalar, int B, int C, int S,
-                             int T, int collapse_last, int quantize, cudaStream_t stream) {
+                             int T, int collapse_last, int quantize, cudaStream_t stream, const float* g = nullptr, float w = 0.f) {
   unsigned grid = 0;
   if (strip_grid(B, C, S, &grid)) return -1;
   const size_t smem = strip_smem<NQ>(S);
   static size_t attr = 0;
-  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_apply_strip_kernel<NQ, kAdj>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
-  blur_apply_strip_kernel<NQ, kAdj><<<grid, kStripThreads, smem, stream>>>(x, out, ops, reinterpret_cast<const long long*>(t), t_scalar,
-                                                                          C, S, T, collapse_last, quantize);
+  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_apply_strip_kernel<NQ, kAdj, kAxpy>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
+  blur_apply_strip_kernel<NQ, kAdj, kAxpy><<<grid, kStripThreads, smem, stream>>>(x, out, ops, reinterpret_cast<const long long*>(t),
+                                                                                 t_scalar, C, S, T, collapse_last, quantize, g, w);
   CD_LAUNCH_CHECK();
   return 0;
 }
 
-template <int NQ>
+template <int NQ, bool kAxpy = false>
 static int blur_step_down_strips(const float* xt, const float* xhat, float* out, const float* ops, int t_hi, int t_lo, int B, int C,
-                                 int S, int T, int collapse_last, cudaStream_t stream) {
+                                 int S, int T, int collapse_last, cudaStream_t stream, const float* g = nullptr, float w = 0.f) {
   unsigned grid = 0;
   if (strip_grid(B, C, S, &grid)) return -1;
   const size_t smem = strip_smem<NQ>(S);
   static size_t attr = 0;
-  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_step_down_strip_kernel<NQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
-  blur_step_down_strip_kernel<NQ><<<grid, kStripThreads, smem, stream>>>(xt, xhat, out, ops, t_hi, t_lo, S, T, collapse_last);
+  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_step_down_strip_kernel<NQ, kAxpy>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
+  blur_step_down_strip_kernel<NQ, kAxpy><<<grid, kStripThreads, smem, stream>>>(xt, xhat, out, ops, t_hi, t_lo, S, T, collapse_last, g, w);
   CD_LAUNCH_CHECK();
   return 0;
 }
 
-// S <= 128: one CTA per plane (blur_apply_kernel / blur_step_down_kernel); 128 < S <= 512: one CTA per row strip
-template <bool kAdj>
+// S <= 128: one CTA per plane (blur_apply_kernel / blur_step_down_kernel); 128 < S <= 512: one CTA per row strip.
+// kEpi: see blur_apply_kernel; kEpiGuide is one-CTA only (cd_blur_guide_grad runs two passes above 128).
+template <bool kAdj, int kEpi = kEpiNone>
 static int blur_apply(const char* name, const float* x, float* out, const float* ops, const int64_t* t, int t_scalar, int B, int C,
-                      int S, int T, int collapse_last, int quantize, cudaStream_t stream) {
+                      int S, int T, int collapse_last, int quantize, cudaStream_t stream, const float* g = nullptr, float w = 0.f) {
   CD_REQUIRE(S % 4 == 0 && S >= 4 && S <= 512, "%s: image size %d unsupported (need S%%4==0, 4<=S<=512)", name, S);
   if (S > 128) {
-    if (S <= 256) return blur_apply_strips<2, kAdj>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, stream);
-    if (S <= 384) return blur_apply_strips<3, kAdj>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, stream);
-    return blur_apply_strips<4, kAdj>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, stream);
+    if constexpr (kEpi == kEpiGuide) {
+      CD_FAIL("%s: the one-pass guidance gradient needs S <= 128", name);
+    } else {
+      constexpr bool kAxpy = kEpi == kEpiAxpy;
+      if (S <= 256) return blur_apply_strips<2, kAdj, kAxpy>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, stream, g, w);
+      if (S <= 384) return blur_apply_strips<3, kAdj, kAxpy>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, stream, g, w);
+      return blur_apply_strips<4, kAdj, kAxpy>(x, out, ops, t, t_scalar, B, C, S, T, collapse_last, quantize, stream, g, w);
+    }
   }
   const size_t smem = blur_smem(S, 2);
   static size_t attr = 0;
-  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_apply_kernel<kAdj>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
+  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_apply_kernel<kAdj, kEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
   dim3 grid(C, B);
-  blur_apply_kernel<kAdj><<<grid, 256, smem, stream>>>(x, out, ops, reinterpret_cast<const long long*>(t), t_scalar, S, T,
-                                                       collapse_last, quantize);
+  blur_apply_kernel<kAdj, kEpi><<<grid, 256, smem, stream>>>(x, out, ops, reinterpret_cast<const long long*>(t), t_scalar, S, T,
+                                                             collapse_last, quantize, g, w);
   CD_LAUNCH_CHECK();
   return 0;
 }
@@ -590,22 +634,56 @@ extern "C" int cd_blur_apply_adjoint(const float* g, float* out, const float* op
                           static_cast<cudaStream_t>(stream));
 }
 
-extern "C" int cd_blur_step_down(const float* xt, const float* xhat, float* out, const float* ops,
-                                 int t_hi, int t_lo, int B, int C, int S, int T, int collapse_last, void* stream) {
-  CD_REQUIRE(S % 4 == 0 && S >= 4 && S <= 512, "cd_blur_step_down: image size %d unsupported (need S%%4==0, 4<=S<=512)", S);
+template <bool kAxpy>
+static int blur_step_down(const char* name, const float* xt, const float* xhat, float* out, const float* ops, int t_hi, int t_lo,
+                          int B, int C, int S, int T, int collapse_last, cudaStream_t st, const float* g, float w) {
+  CD_REQUIRE(S % 4 == 0 && S >= 4 && S <= 512, "%s: image size %d unsupported (need S%%4==0, 4<=S<=512)", name, S);
   if (S > 128) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (S <= 256) return blur_step_down_strips<2>(xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, collapse_last, st);
-    if (S <= 384) return blur_step_down_strips<3>(xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, collapse_last, st);
-    return blur_step_down_strips<4>(xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, collapse_last, st);
+    if (S <= 256) return blur_step_down_strips<2, kAxpy>(xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, collapse_last, st, g, w);
+    if (S <= 384) return blur_step_down_strips<3, kAxpy>(xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, collapse_last, st, g, w);
+    return blur_step_down_strips<4, kAxpy>(xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, collapse_last, st, g, w);
   }
   const size_t smem = blur_smem(S, 2);
   static size_t attr = 0;
-  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_step_down_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
+  if (smem > attr) { CD_CUDA(cudaFuncSetAttribute(blur_step_down_kernel<kAxpy>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = smem; }
   dim3 grid(C, B);
-  blur_step_down_kernel<<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(xt, xhat, out, ops, t_hi, t_lo, S, T, collapse_last);
+  blur_step_down_kernel<kAxpy><<<grid, 256, smem, st>>>(xt, xhat, out, ops, t_hi, t_lo, S, T, collapse_last, g, w);
   CD_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int cd_blur_step_down(const float* xt, const float* xhat, float* out, const float* ops,
+                                 int t_hi, int t_lo, int B, int C, int S, int T, int collapse_last, void* stream) {
+  return blur_step_down<false>("cd_blur_step_down", xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, collapse_last,
+                               static_cast<cudaStream_t>(stream), nullptr, 0.f);
+}
+
+// ---- guided restoration (GaussianDiffusion.restore) ----------------------------------------------------------------------
+// the guidance gradient D^T (D x0 - y) of D = A_idx (.) A_idx^T: one pass up to 128² (the residual never leaves shared memory),
+// two above (the apply kernel with a "- y" epilogue into `work`, then the adjoint kernel)
+extern "C" int cd_blur_guide_grad(const float* x0, const float* y, float* out, float* work, const float* ops, int idx,
+                                  int B, int C, int S, int T, void* stream) {
+  CD_REQUIRE(x0 && y && out && ops && idx < T && B >= 1 && C >= 1, "cd_blur_guide_grad: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (S <= 128)
+    return blur_apply<false, kEpiGuide>("cd_blur_guide_grad", x0, out, ops, nullptr, idx, B, C, S, T, 0, 0, st, y, 1.f);
+  CD_REQUIRE(work && work != out, "cd_blur_guide_grad: S = %d > 128 needs a workspace of B*C*S*S floats apart from out", S);
+  if (blur_apply<false, kEpiAxpy>("cd_blur_guide_grad", x0, work, ops, nullptr, idx, B, C, S, T, 0, 0, st, y, 1.f)) return -1;
+  return blur_apply<true>("cd_blur_guide_grad", work, out, ops, nullptr, idx, B, C, S, T, 0, 0, st);
+}
+
+// the guided update: xt == NULL -> `default`, out = D(xhat, t_lo) - w g; else `x0_step_down`, out = xt - D(xhat, t_hi) +
+// D(xhat, t_lo) - w g.  g == NULL runs the unguided kernels themselves (their bits).
+extern "C" int cd_blur_guided_step(const float* xt, const float* xhat, const float* g, float weight, float* out, const float* ops,
+                                   int t_hi, int t_lo, int B, int C, int S, int T, void* stream) {
+  CD_REQUIRE(xhat && out && ops && t_hi < T && t_lo < T, "cd_blur_guided_step: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!xt) {
+    if (!g) return blur_apply<false>("cd_blur_guided_step", xhat, out, ops, nullptr, t_lo, B, C, S, T, 0, 0, st);
+    return blur_apply<false, kEpiAxpy>("cd_blur_guided_step", xhat, out, ops, nullptr, t_lo, B, C, S, T, 0, 0, st, g, weight);
+  }
+  if (!g) return blur_step_down<false>("cd_blur_guided_step", xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, 0, st, nullptr, 0.f);
+  return blur_step_down<true>("cd_blur_guided_step", xt, xhat, out, ops, t_hi, t_lo, B, C, S, T, 0, st, g, weight);
 }
 
 extern "C" int cd_loss_fwd_bwd(const float* x0, const float* xhat, int64_t n, int mode, float grad_scale,
@@ -893,23 +971,32 @@ __device__ __forceinline__ float quantize8(float v) {            // DFG:380-384 
   q = static_cast<float>(static_cast<int>(q)) / 255.f;
   return q * 2.f - 1.f;
 }
+// kEpi (guided restoration; quantize is then 0): kEpiAxpy out = x m - w g (the guided `default` update); kEpiGuide out =
+// m (x m - g), the guidance gradient with g = y
+template <int kEpi = kEpiNone>
 __global__ void mask_apply_kernel(const float* __restrict__ x, float* __restrict__ out, const float* __restrict__ masks,
                                   const long long* __restrict__ t, int t_scalar, const long long* __restrict__ rx,
-                                  const long long* __restrict__ ry, int B, int C, int S, int MS, int quantize) {
+                                  const long long* __restrict__ ry, int B, int C, int S, int MS, int quantize,
+                                  const float* __restrict__ g, float w) {
   const long long n = static_cast<long long>(B) * C * S * S;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int xx = static_cast<int>(i % S), yy = static_cast<int>((i / S) % S);
     const int b = static_cast<int>(i / (static_cast<long long>(S) * S * C));
     const int idx = t ? static_cast<int>(t[b]) : t_scalar;
     const int oy = rx ? static_cast<int>(rx[b]) : 0, ox = ry ? static_cast<int>(ry[b]) : 0;   // reference: rows <- rand_x, cols <- rand_y
-    float v = x[i] * mask_at(masks, idx, MS, yy + oy, xx + ox);
+    const float m = mask_at(masks, idx, MS, yy + oy, xx + ox);
+    float v = x[i] * m;
+    if constexpr (kEpi == kEpiAxpy) v = v - w * g[i];
+    if constexpr (kEpi == kEpiGuide) v = (v - g[i]) * m;
     if (quantize) v = quantize8(v);
     out[i] = v;
   }
 }
+template <bool kAxpy = false>
 __global__ void mask_step_down_kernel(const float* __restrict__ xt, const float* __restrict__ xhat, float* __restrict__ out,
                                       const float* __restrict__ masks, int idx_hi, int idx_lo, const long long* __restrict__ rx,
-                                      const long long* __restrict__ ry, int B, int C, int S, int MS) {
+                                      const long long* __restrict__ ry, int B, int C, int S, int MS, const float* __restrict__ g,
+                                      float w) {
   const long long n = static_cast<long long>(B) * C * S * S;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int xx = static_cast<int>(i % S), yy = static_cast<int>((i / S) % S);
@@ -918,29 +1005,66 @@ __global__ void mask_step_down_kernel(const float* __restrict__ xt, const float*
     const float xv = xhat[i];
     const float hi = xv * mask_at(masks, idx_hi, MS, yy + oy, xx + ox);
     const float lo = xv * mask_at(masks, idx_lo, MS, yy + oy, xx + ox);
-    out[i] = xt[i] - hi + lo;
+    float v = xt[i] - hi + lo;
+    if constexpr (kAxpy) v = v - w * g[i];
+    out[i] = v;
   }
+}
+
+template <int kEpi>
+int mask_apply(const float* x, float* out, const float* masks, const int64_t* t, int t_scalar, const int64_t* rx, const int64_t* ry,
+               int B, int C, int S, int MS, int quantize, cudaStream_t stream, const float* g, float w) {
+  const long long n = static_cast<long long>(B) * C * S * S;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
+  mask_apply_kernel<kEpi><<<blocks, 256, 0, stream>>>(x, out, masks, reinterpret_cast<const long long*>(t), t_scalar,
+      reinterpret_cast<const long long*>(rx), reinterpret_cast<const long long*>(ry), B, C, S, MS, quantize, g, w);
+  CD_LAUNCH_CHECK();
+  return 0;
+}
+
+template <bool kAxpy>
+int mask_step_down(const float* xt, const float* xhat, float* out, const float* masks, int idx_hi, int idx_lo, const int64_t* rx,
+                   const int64_t* ry, int B, int C, int S, int MS, cudaStream_t stream, const float* g, float w) {
+  const long long n = static_cast<long long>(B) * C * S * S;
+  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
+  mask_step_down_kernel<kAxpy><<<blocks, 256, 0, stream>>>(xt, xhat, out, masks, idx_hi, idx_lo,
+      reinterpret_cast<const long long*>(rx), reinterpret_cast<const long long*>(ry), B, C, S, MS, g, w);
+  CD_LAUNCH_CHECK();
+  return 0;
 }
 }  // namespace
 
 extern "C" int cd_mask_apply(const float* x, float* out, const float* masks, const int64_t* t, int t_scalar,
                              const int64_t* rx, const int64_t* ry, int B, int C, int S, int MS, int quantize, void* stream) {
-  const long long n = static_cast<long long>(B) * C * S * S;
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
-  mask_apply_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, out, masks, reinterpret_cast<const long long*>(t), t_scalar,
-      reinterpret_cast<const long long*>(rx), reinterpret_cast<const long long*>(ry), B, C, S, MS, quantize);
-  CD_LAUNCH_CHECK();
-  return 0;
+  return mask_apply<kEpiNone>(x, out, masks, t, t_scalar, rx, ry, B, C, S, MS, quantize, static_cast<cudaStream_t>(stream), nullptr, 0.f);
 }
 
 extern "C" int cd_mask_step_down(const float* xt, const float* xhat, float* out, const float* masks, int idx_hi, int idx_lo,
                                  const int64_t* rx, const int64_t* ry, int B, int C, int S, int MS, void* stream) {
-  const long long n = static_cast<long long>(B) * C * S * S;
-  int blocks = cd_cdiv(n, 256 * 4); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
-  mask_step_down_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(xt, xhat, out, masks, idx_hi, idx_lo,
-      reinterpret_cast<const long long*>(rx), reinterpret_cast<const long long*>(ry), B, C, S, MS);
-  CD_LAUNCH_CHECK();
-  return 0;
+  return mask_step_down<false>(xt, xhat, out, masks, idx_hi, idx_lo, rx, ry, B, C, S, MS, static_cast<cudaStream_t>(stream), nullptr,
+                               0.f);
+}
+
+// guided restoration: the guidance gradient m (m x0 - y) with m = the mask at idx in each sample's window, in one pass
+extern "C" int cd_mask_guide_grad(const float* x0, const float* y, float* out, const float* masks, int idx, const int64_t* rx,
+                                  const int64_t* ry, int B, int C, int S, int MS, void* stream) {
+  CD_REQUIRE(x0 && y && out && masks && B >= 0 && C >= 1 && S >= 1 && MS >= S, "cd_mask_guide_grad: bad arguments");
+  return mask_apply<kEpiGuide>(x0, out, masks, nullptr, idx, rx, ry, B, C, S, MS, 0, static_cast<cudaStream_t>(stream), y, 1.f);
+}
+
+// the guided update: xt == NULL -> `default`, out = xhat m_lo - w g; else out = xt - xhat m_hi + xhat m_lo - w g.  g == NULL runs
+// the unguided kernels themselves (their bits).
+extern "C" int cd_mask_guided_step(const float* xt, const float* xhat, const float* g, float weight, float* out, const float* masks,
+                                   int idx_hi, int idx_lo, const int64_t* rx, const int64_t* ry, int B, int C, int S, int MS,
+                                   void* stream) {
+  CD_REQUIRE(xhat && out && masks && B >= 0 && C >= 1 && S >= 1 && MS >= S, "cd_mask_guided_step: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!xt) {
+    if (!g) return mask_apply<kEpiNone>(xhat, out, masks, nullptr, idx_lo, rx, ry, B, C, S, MS, 0, st, nullptr, 0.f);
+    return mask_apply<kEpiAxpy>(xhat, out, masks, nullptr, idx_lo, rx, ry, B, C, S, MS, 0, st, g, weight);
+  }
+  if (!g) return mask_step_down<false>(xt, xhat, out, masks, idx_hi, idx_lo, rx, ry, B, C, S, MS, st, nullptr, 0.f);
+  return mask_step_down<true>(xt, xhat, out, masks, idx_hi, idx_lo, rx, ry, B, C, S, MS, st, g, weight);
 }
 
 // -------------------------------------------------------------------------------------------------------------
@@ -952,9 +1076,12 @@ extern "C" int cd_mask_step_down(const float* xt, const float* xhat, float* out,
 //  * snow: D depends on the clean image only (FP:361-372): clip(bright_i(og) + snow_i + rot180(snow_i), 0, 1)*2-1.
 // -------------------------------------------------------------------------------------------------------------
 namespace {
+// kEpi (guided restoration): kEpiAxpy = either mode's result - w g; kEpiGuide = the guidance gradient M^T (M xsrc - g) with
+// M = mats[t_hi+hi_off] (mode 0 only; index < 0: xsrc - g)
+template <int kEpi = kEpiNone>
 __global__ void chanmix_kernel(const float* __restrict__ xt, const float* __restrict__ xsrc, float* __restrict__ out,
                                const float* __restrict__ mats, const long long* __restrict__ t_hi, const long long* __restrict__ t_lo,
-                               int hi_off, int lo_off, int B, int C, long long HW, int mode) {
+                               int hi_off, int lo_off, int B, int C, long long HW, int mode, const float* __restrict__ g, float w) {
   // mode 0: out = M[t_hi+hi_off] xsrc ; mode 1: out = xt - M[t_hi+hi_off] xsrc + M[t_lo+lo_off] xsrc   (index < 0 = identity)
   const long long n = static_cast<long long>(B) * HW;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -964,12 +1091,28 @@ __global__ void chanmix_kernel(const float* __restrict__ xt, const float* __rest
     const int il = mode ? static_cast<int>(t_lo[b]) + lo_off : -1;
     float v[8];
     for (int c = 0; c < C; ++c) v[c] = xsrc[(static_cast<long long>(b) * C + c) * HW + p];
-    for (int co = 0; co < C; ++co) {
-      float hi = v[co], lo = v[co];
-      if (ih >= 0) { hi = 0.f; for (int c = 0; c < C; ++c) hi = fmaf(mats[(ih * C + co) * C + c], v[c], hi); }
-      if (il >= 0) { lo = 0.f; for (int c = 0; c < C; ++c) lo = fmaf(mats[(il * C + co) * C + c], v[c], lo); }
-      const long long o = (static_cast<long long>(b) * C + co) * HW + p;
-      out[o] = mode ? xt[o] - hi + lo : hi;
+    if constexpr (kEpi == kEpiGuide) {
+      float r[8];
+      for (int co = 0; co < C; ++co) {
+        float hi = v[co];
+        if (ih >= 0) { hi = 0.f; for (int c = 0; c < C; ++c) hi = fmaf(mats[(ih * C + co) * C + c], v[c], hi); }
+        r[co] = hi - g[(static_cast<long long>(b) * C + co) * HW + p];
+      }
+      for (int c = 0; c < C; ++c) {
+        float s = r[c];
+        if (ih >= 0) { s = 0.f; for (int co = 0; co < C; ++co) s = fmaf(mats[(ih * C + co) * C + c], r[co], s); }
+        out[(static_cast<long long>(b) * C + c) * HW + p] = s;
+      }
+    } else {
+      for (int co = 0; co < C; ++co) {
+        float hi = v[co], lo = v[co];
+        if (ih >= 0) { hi = 0.f; for (int c = 0; c < C; ++c) hi = fmaf(mats[(ih * C + co) * C + c], v[c], hi); }
+        if (il >= 0) { lo = 0.f; for (int c = 0; c < C; ++c) lo = fmaf(mats[(il * C + co) * C + c], v[c], lo); }
+        const long long o = (static_cast<long long>(b) * C + co) * HW + p;
+        float r = mode ? xt[o] - hi + lo : hi;
+        if constexpr (kEpi == kEpiAxpy) r = r - w * g[o];
+        out[o] = r;
+      }
     }
   }
 }
@@ -1007,15 +1150,41 @@ __global__ void snow_kernel(const float* __restrict__ xt, const float* __restric
 }
 }  // namespace
 
+namespace {
+template <int kEpi>
+int chanmix(const float* xt, const float* xsrc, float* out, const float* mats, const int64_t* t_hi, const int64_t* t_lo, int hi_off,
+            int lo_off, int B, int C, int64_t HW, int mode, cudaStream_t stream, const float* g, float w) {
+  const long long n = static_cast<long long>(B) * HW;
+  int blocks = cd_cdiv(n, 256 * 2); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
+  chanmix_kernel<kEpi><<<blocks, 256, 0, stream>>>(xt, xsrc, out, mats, reinterpret_cast<const long long*>(t_hi),
+      reinterpret_cast<const long long*>(t_lo), hi_off, lo_off, B, C, HW, mode, g, w);
+  CD_LAUNCH_CHECK();
+  return 0;
+}
+}  // namespace
+
 extern "C" int cd_chanmix(const float* xt, const float* xsrc, float* out, const float* mats, const int64_t* t_hi,
                           const int64_t* t_lo, int hi_off, int lo_off, int B, int C, int64_t HW, int mode, void* stream) {
   CD_REQUIRE(C <= 8 && t_hi && (mode == 0 || (xt && t_lo)), "cd_chanmix: bad arguments");
-  const long long n = static_cast<long long>(B) * HW;
-  int blocks = cd_cdiv(n, 256 * 2); if (blocks > cd_num_sms() * 8) blocks = cd_num_sms() * 8; if (blocks < 1) blocks = 1;
-  chanmix_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(xt, xsrc, out, mats, reinterpret_cast<const long long*>(t_hi),
-      reinterpret_cast<const long long*>(t_lo), hi_off, lo_off, B, C, HW, mode);
-  CD_LAUNCH_CHECK();
-  return 0;
+  return chanmix<kEpiNone>(xt, xsrc, out, mats, t_hi, t_lo, hi_off, lo_off, B, C, HW, mode, static_cast<cudaStream_t>(stream), nullptr,
+                           0.f);
+}
+
+// guided restoration: the guidance gradient M^T (M x0 - y) per pixel, M = mats[t[b] + off] (index < 0: x0 - y), in one pass
+extern "C" int cd_chanmix_guide_grad(const float* x0, const float* y, float* out, const float* mats, const int64_t* t, int off,
+                                     int B, int C, int64_t HW, void* stream) {
+  CD_REQUIRE(x0 && y && out && mats && t && C >= 1 && C <= 8 && B >= 0 && HW >= 0, "cd_chanmix_guide_grad: bad arguments");
+  return chanmix<kEpiGuide>(nullptr, x0, out, mats, t, nullptr, off, 0, B, C, HW, 0, static_cast<cudaStream_t>(stream), y, 1.f);
+}
+
+// the guided update: cd_chanmix's mode 0 / 1 result - w g.  g == NULL runs cd_chanmix itself (its bits).
+extern "C" int cd_chanmix_guided(const float* xt, const float* xsrc, const float* g, float weight, float* out, const float* mats,
+                                 const int64_t* t_hi, const int64_t* t_lo, int hi_off, int lo_off, int B, int C, int64_t HW, int mode,
+                                 void* stream) {
+  CD_REQUIRE(C <= 8 && t_hi && (mode == 0 || (mode == 1 && xt && t_lo)), "cd_chanmix_guided: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!g) return chanmix<kEpiNone>(xt, xsrc, out, mats, t_hi, t_lo, hi_off, lo_off, B, C, HW, mode, st, nullptr, 0.f);
+  return chanmix<kEpiAxpy>(xt, xsrc, out, mats, t_hi, t_lo, hi_off, lo_off, B, C, HW, mode, st, g, weight);
 }
 
 extern "C" int cd_snow(const float* xt, const float* og, float* out, const float* snow, const float* br_coef, const int64_t* t_hi,

@@ -14,6 +14,7 @@ import torch.nn.functional as F  # noqa: F401  (kept for API familiarity; not us
 from ._lib import call, ptr, stream
 from .autograd import BlurDegrade, refuse_grad
 from .degradation import build_blur_operators
+from .guided import check_arguments, refuse_restore, restore_loop
 from .strided import refuse_strided, reverse_levels
 
 
@@ -206,6 +207,46 @@ class GaussianDiffusion(nn.Module):
             img = x
         self.denoise_fn.train()
         return xt, direct_recons, img
+
+    def restore(self, y, s, *, weight, steps=None):
+        """guided restoration (guided.py): Algorithm 2 from the observation y = D_s(x) through the levels of
+        strided.reverse_levels(s, steps), each step pulled towards D_s(x0_hat) = y with the guidance weight.  D_s is what
+        `sample(img=x, t=s)` applies to x: the cumulative operator s - 1 (Individual_Incremental: the single kernel (s - 1) % T).
+        weight = 0 is `sample(img=x, t=s, steps=steps)`'s final image bit for bit.  Raises ValueError for `discrete` and for
+        the routines `sample(steps=K)` refuses."""
+        if self.discrete:
+            refuse_restore('deblurring', "discrete=True (the 8-bit truncation has no gradient)")
+        try:
+            self._check_strided(1)           # the routines without a strided form
+        except ValueError:
+            refuse_restore('deblurring', "train_routine=%r, sampling_routine=%r, blur_routine=%r (no strided form)" % (
+                self.train_routine, self.sampling_routine, self.blur_routine))
+        check_arguments('deblurring', y, s, weight, self.num_timesteps, (self.channels, self.image_size, self.image_size))
+        s, weight = int(s), float(weight)
+        levels = reverse_levels(s, steps)
+        y = y.contiguous()
+        B, Cc, S, _ = y.shape
+        T = self.num_timesteps
+        single = self.blur_routine == 'Individual_Incremental'
+        obs_ops, obs_idx = (self._ops_single, (s - 1) % T) if single else (self._ops_cum, s - 1)
+        work = torch.empty_like(y) if S > 128 and weight > 0 else None
+
+        def guide_grad(x0):
+            out = torch.empty_like(x0)
+            call('cd_blur_guide_grad', ptr(x0), ptr(y), ptr(out), ptr(work), ptr(obs_ops), obs_idx, B, Cc, S, T, stream())
+            return out
+
+        def step(img, x0, g, hi, lo):
+            out = torch.empty_like(img)
+            xt = img.contiguous() if self.sampling_routine == 'x0_step_down' else None
+            call('cd_blur_guided_step', ptr(xt), ptr(x0.contiguous()), ptr(g), C.c_float(weight), ptr(out), ptr(self._ops_cum),
+                 hi - 1, lo - 1, B, Cc, S, T, stream())
+            return out
+
+        self.denoise_fn.eval()
+        img = restore_loop(self.denoise_fn, y, levels, weight, guide_grad, step)
+        self.denoise_fn.train()
+        return img
 
     @torch.no_grad()
     def gen_sample(self, batch_size=16, img=None, t=None, noise_level=0):

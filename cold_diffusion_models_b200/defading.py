@@ -13,6 +13,7 @@ from ._lib import call, ptr, stream
 from .autograd import MaskDegrade, refuse_grad
 from .deblurring import _LossFn
 from .degradation import gaussian_taps
+from .guided import check_arguments, refuse_restore, restore_loop
 from .strided import refuse_strided, reverse_levels
 
 
@@ -138,6 +139,38 @@ class GaussianDiffusion(nn.Module):
                 x = out
             recon = x
         return xt, direct_recons, recon
+
+    def restore(self, y, s, *, weight, steps=None, _offsets=None):
+        """guided restoration (guided.py) from the observation y = D_s(x) = x * mask_{s-1}, the fade `sample(faded_recon_sample=x,
+        t=s)` applies, in each sample's window of the 'Random_*' routines (`_offsets`, as `sample` takes them; drawn when None).
+        weight = 0 is `sample`'s final image bit for bit.  Raises ValueError for `discrete` and for the routines
+        `sample(steps=K)` refuses."""
+        if self.discrete:
+            refuse_restore('defading', "discrete=True (the 8-bit truncation has no gradient)")
+        if self.sampling_routine not in ('default', 'x0_step_down'):
+            refuse_restore('defading', "sampling_routine=%r (no strided form)" % self.sampling_routine)
+        check_arguments('defading', y, s, weight, self.num_timesteps, (self.channels, self.image_size, self.image_size))
+        s, weight = int(s), float(weight)
+        levels = reverse_levels(s, steps)
+        y = y.contiguous()
+        B, Cc, S, _ = y.shape
+        MS = self._masks_cum.shape[-1]
+        rx, ry = _offsets if _offsets is not None else self._offsets(B, y.device)
+
+        def guide_grad(x0):
+            out = torch.empty_like(x0)
+            call('cd_mask_guide_grad', ptr(x0), ptr(y), ptr(out), ptr(self._masks_cum), s - 1, ptr(rx), ptr(ry), B, Cc, S, MS,
+                 stream())
+            return out
+
+        def step(img, x0, g, hi, lo):
+            out = torch.empty_like(img)
+            xt = img.contiguous() if self.sampling_routine == 'x0_step_down' else None
+            call('cd_mask_guided_step', ptr(xt), ptr(x0.contiguous()), ptr(g), C.c_float(weight), ptr(out), ptr(self._masks_cum),
+                 hi - 1, lo - 1, ptr(rx), ptr(ry), B, Cc, S, MS, stream())
+            return out
+
+        return restore_loop(self.defade_fn, y, levels, weight, guide_grad, step)
 
     @torch.no_grad()
     def all_sample(self, batch_size=16, faded_recon_sample=None, t=None, times=None, _offsets=None):

@@ -18,6 +18,7 @@ from ._lib import call, ptr, stream
 from .autograd import BlurDegrade
 from .deblurring import _LossFn
 from .degradation import gaussian_taps, blur_matrix
+from .guided import check_arguments, refuse_restore, restore_loop
 from .strided import refuse_strided, reverse_levels
 
 
@@ -238,6 +239,36 @@ class GaussianDiffusion(nn.Module):
                 x = self._reverse_step(img, x, hi, lo)
             img = x
         return xt, direct_recons, img
+
+    def restore(self, y, s, *, weight, steps=None):
+        """guided restoration (guided.py) from the observation y = D_s(x), D_s = the tabulated cumulative operator s - 1 that
+        `sample(img=x, t=s)` applies.  weight = 0 is `sample(img=x, t=s, steps=steps)`'s final image bit for bit.  Raises
+        ValueError for the routines `sample(steps=K)` refuses."""
+        if self.train_routine != 'Final':
+            refuse_restore('resolution', "train_routine=%r (no strided form)" % self.train_routine)
+        if self.sampling_routine not in ('default', 'x0_step_down'):
+            refuse_restore('resolution', "sampling_routine=%r (no strided form)" % self.sampling_routine)
+        check_arguments('resolution', y, s, weight, self.num_timesteps, (self.channels, self.image_size, self.image_size))
+        s, weight = int(s), float(weight)
+        levels = reverse_levels(s, steps)
+        y = y.contiguous()
+        B, Cc, S, _ = y.shape
+        T = self.num_timesteps
+        work = torch.empty_like(y) if S > 128 and weight > 0 else None
+
+        def guide_grad(x0):
+            out = torch.empty_like(x0)
+            call('cd_blur_guide_grad', ptr(x0), ptr(y), ptr(out), ptr(work), ptr(self._ops_cum), s - 1, B, Cc, S, T, stream())
+            return out
+
+        def step(img, x0, g, hi, lo):
+            out = torch.empty_like(img)
+            xt = img.contiguous() if self.sampling_routine == 'x0_step_down' else None
+            call('cd_blur_guided_step', ptr(xt), ptr(x0.contiguous()), ptr(g), C.c_float(weight), ptr(out), ptr(self._ops_cum),
+                 hi - 1, lo - 1, B, Cc, S, T, stream())
+            return out
+
+        return restore_loop(self.denoise_fn, y, levels, weight, guide_grad, step)
 
     @torch.no_grad()
     def opt(self, img, t=None):

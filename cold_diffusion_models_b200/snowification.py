@@ -27,6 +27,7 @@ from ._lib import call, ptr, stream
 from .autograd import ChanmixDegrade, refuse_grad
 from .deblurring import _LossFn
 from .degradation import gaussian_taps
+from .guided import check_arguments, refuse_restore, restore_loop
 from .strided import refuse_strided, reverse_levels
 from .train_graph import recording
 
@@ -435,6 +436,51 @@ class GaussianDiffusion(nn.Module):
         if self.to_lab:                                                             # SN:287-290
             xt, direct_recons, img = lab2rgb(xt), lab2rgb(direct_recons), lab2rgb(img)
         return {'xt': xt, 'direct_recons': direct_recons, 'recon': img}
+
+    def restore(self, y, s, *, weight, steps=None):
+        """guided restoration (guided.py) for decolorization without Lab, from the observation y = D_s(x) = M_{s-1} x per pixel,
+        the mix `sample(img=x, t=s)` applies.  The updates index D one step lower, as `sample_one_step` does: 'default' x_lo =
+        M_{lo-2} x0_hat - weight g, 'x0_step_down' x_lo = x_hi - M_{hi-2} x0_hat + M_{lo-2} x0_hat - weight g (index < 0:
+        identity).  weight = 0 is `sample(img=x, t=s, steps=steps)['recon']` bit for bit.  Raises ValueError for snow and the
+        Lab path (nonlinear and clipped) and for the routines `sample(steps=K)` refuses."""
+        if not isinstance(self.forward_process, DeColorization):
+            refuse_restore('snowification', "snow (nonlinear and clipped)")
+        if self.to_lab:
+            refuse_restore('snowification', "the Lab decolor path (nonlinear and clipped)")
+        if self.train_routine not in self._FINAL_ROUTINES:
+            refuse_restore('snowification', "train_routine=%r (no strided form)" % self.train_routine)
+        if self.sampling_routine not in ('default', 'x0_step_down'):
+            refuse_restore('snowification', "sampling_routine=%r (no strided form)" % self.sampling_routine)
+        hw = tuple(self.image_size) if isinstance(self.image_size, tuple) else (self.image_size, self.image_size)
+        check_arguments('snowification', y, s, weight, self.num_timesteps, (self.channels,) + hw)
+        s, weight = int(s), float(weight)
+        levels = reverse_levels(s, steps)
+        y = y.contiguous()
+        B, Cc, H, W = y.shape
+        mats = self._tab(y.device)[1]
+        level = lambda n: torch.full((B,), n, dtype=torch.long, device=y.device)
+        t_obs = level(s)
+
+        def guide_grad(x0):
+            out = torch.empty_like(x0)
+            call('cd_chanmix_guide_grad', ptr(x0), ptr(y), ptr(out), ptr(mats), ptr(t_obs), -1, B, Cc, C.c_int64(H * W), stream())
+            return out
+
+        def step(img, x0, g, hi, lo):
+            out = torch.empty_like(img)
+            x0 = x0.contiguous()
+            t_hi, t_lo = level(hi - 1), level(lo - 1)
+            if self.sampling_routine == 'default':
+                call('cd_chanmix_guided', ptr(None), ptr(x0), ptr(g), C.c_float(weight), ptr(out), ptr(mats), ptr(t_lo),
+                     ptr(None), -1, 0, B, Cc, C.c_int64(H * W), 0, stream())
+                return out
+            if self.recon_noise_std > 0.0:                     # as sample_one_step
+                x0 = x0 + torch.normal(0.0, self.recon_noise_std, size=x0.size(), device=x0.device)
+            call('cd_chanmix_guided', ptr(img.contiguous()), ptr(x0), ptr(g), C.c_float(weight), ptr(out), ptr(mats),
+                 ptr(t_hi), ptr(t_lo), -1, -1, B, Cc, C.c_int64(H * W), 1, stream())
+            return out
+
+        return restore_loop(self.denoise_fn, y, levels, weight, guide_grad, step)
 
     def _total_forward(self, img):
         """forward_process.total_forward: decolor = every channel <- channel mean (FP:198-218, independent of the schedule),

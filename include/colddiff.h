@@ -333,6 +333,29 @@ int cd_mask_step_down(const float* xt, const float* xhat, float* out, const floa
  * rot180(snow_i), 0, 1)*2-1 with snow [T][snow_batch][3][H][W] (FP:361-372).                                                   */
 int cd_chanmix(const float* xt, const float* xsrc, float* out, const float* mats, const int64_t* t_hi,
                const int64_t* t_lo, int hi_off, int lo_off, int B, int C, int64_t HW, int mode, void* stream);
+/* Guided restoration (`GaussianDiffusion.restore`): reconstruction guidance for the linear degradations D_s.
+ * Guidance gradient in image space, ghat = D_s^T (D_s x0 - y), fp32 NCHW, one entry point per family:
+ *   cd_blur_guide_grad    : D_s = A_idx (.) A_idx^T per plane (idx < 0: identity), the cd_blur_apply operator table.  S <= 128
+ *                           runs one pass (the residual stays on chip); 128 < S <= 512 runs cd_blur_apply with a "- y" epilogue
+ *                           into `work` (B*C*S*S floats, not `out`), then the adjoint.  Same size rule as cd_blur_apply.
+ *   cd_mask_guide_grad    : m (m x0 - y), m = masks[idx] in each sample's window (rx / ry as cd_mask_apply), one pass.
+ *   cd_chanmix_guide_grad : M^T (M x0 - y) per pixel, M = mats[t[b] + off] (index < 0: x0 - y), one pass.
+ * Guided update: the reverse step with "- weight * g" in its epilogue.  xt == NULL (mask, blur) or mode 0 (chanmix): the `default`
+ * update D(xhat, lo) - weight g; otherwise `x0_step_down`, xt - D(xhat, hi) + D(xhat, lo) - weight g.  Indices as in
+ * cd_blur_apply / cd_blur_step_down, cd_mask_step_down and cd_chanmix.  g == NULL runs the unguided kernel itself, bit for bit. */
+int cd_blur_guide_grad(const float* x0, const float* y, float* out, float* work, const float* ops, int idx,
+                       int B, int C, int S, int T, void* stream);
+int cd_blur_guided_step(const float* xt, const float* xhat, const float* g, float weight, float* out, const float* ops,
+                        int t_hi, int t_lo, int B, int C, int S, int T, void* stream);
+int cd_mask_guide_grad(const float* x0, const float* y, float* out, const float* masks, int idx, const int64_t* rx,
+                       const int64_t* ry, int B, int C, int S, int MS, void* stream);
+int cd_mask_guided_step(const float* xt, const float* xhat, const float* g, float weight, float* out, const float* masks,
+                        int idx_hi, int idx_lo, const int64_t* rx, const int64_t* ry, int B, int C, int S, int MS, void* stream);
+int cd_chanmix_guide_grad(const float* x0, const float* y, float* out, const float* mats, const int64_t* t, int off,
+                          int B, int C, int64_t HW, void* stream);
+int cd_chanmix_guided(const float* xt, const float* xsrc, const float* g, float weight, float* out, const float* mats,
+                      const int64_t* t_hi, const int64_t* t_lo, int hi_off, int lo_off, int B, int C, int64_t HW, int mode,
+                      void* stream);
 int cd_snow(const float* xt, const float* og, float* out, const float* snow, const float* br_coef, const int64_t* t_hi,
             const int64_t* t_lo, int hi_off, int lo_off, int B, int H, int W, int snow_batch, int fix_brightness,
             int mode, void* stream);
